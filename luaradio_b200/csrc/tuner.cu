@@ -21,8 +21,9 @@
 // padded by 2 samples every R*D, which makes the per-thread stride (R*D+2)*8 B conflict-free for 128-bit loads.
 //
 // Rotation.  x[i] e^{jw(g0+i)} = P_tile * (x[i] * E[i - B]) with E the tile-relative phasor and P_tile the phasor of
-// the tile origin.  E is applied while staging: a thread always stages the same tile-relative sample pairs, so
-// E[2u] = A0 * step[it] with A0 = E[2 tid] held in registers for the whole (persistent) kernel and step[it] a
+// the tile origin.  E is applied while staging: a thread always stages the same tile-relative sample pairs, so the
+// interior kernel keeps E of the first sample of each of its pairs in registers for the whole (persistent) kernel and
+// derives the second as E * e^{jw}; the edge kernel forms E[2u] = A0 * step[it] with A0 = E[2 tid] and step[it] a
 // per-iteration constant from the constant bank -- no table stream, no transcendental per sample.  P_tile commutes
 // with the filter and is applied to the 1/D kept outputs (not at all under the fused discriminator, which only
 // sees y[m] conj(y[m-1])).
@@ -96,7 +97,37 @@ struct PolyShape {
     __host__ __device__ static constexpr int pad(int e) { return e + 2 * (e / RD); }
     static constexpr int ELEMS = LOADED + 2 * (LOADED / RD) + 2;
     static constexpr size_t SMEM = (size_t)ELEMS * sizeof(float2);
+    // bulk-copied interior tiles: the tile lands unpadded behind the padded one (RAW), and the rotation pass moves it into
+    // the padded layout, RD-sample segment by segment (stride RD + 2): each of RG thread groups takes one segment per
+    // pass, a thread one sample pair of it
+    static constexpr int RAW = ELEMS;
+    static constexpr size_t SMEM_BULK = (size_t)(ELEMS + LOADED) * sizeof(float2);
+    static constexpr int NSEG = (LOADED + RD - 1) / RD;
+    static constexpr int PPS = RD / 2;                            // sample pairs per segment
+    static constexpr int RG = PT_THREADS / PPS;
+    static constexpr int RITERS = (NSEG + RG - 1) / RG;
 };
+
+// ---- cp.async.bulk (global -> shared, completion counted in bytes on an mbarrier)
+__device__ __forceinline__ uint32_t smem_addr(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
+__device__ __forceinline__ void mbar_init(uint64_t* bar) {
+    asm volatile("mbarrier.init.shared::cta.b64 [%0], 1;\n\tfence.mbarrier_init.release.cluster;\n\t"
+                 "fence.proxy.async.shared::cta;" :: "r"(smem_addr(bar)) : "memory");
+}
+__device__ __forceinline__ void mbar_expect_tx(uint64_t* bar, uint32_t bytes) {
+    asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" :: "r"(smem_addr(bar)), "r"(bytes) : "memory");
+}
+__device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
+    asm volatile("{\n\t.reg .pred p;\n\tLRB_WAIT_%=:\n\t"
+                 "mbarrier.try_wait.parity.shared::cta.b64 p, [%0], %1;\n\t"
+                 "@!p bra LRB_WAIT_%=;\n\t}" :: "r"(smem_addr(bar)), "r"(parity) : "memory");
+}
+// orders this thread's earlier generic-proxy accesses of shared memory before its later bulk copies into it
+__device__ __forceinline__ void fence_proxy_async() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
+__device__ __forceinline__ void bulk_g2s(void* dst, const void* src, uint32_t bytes, uint64_t* bar) {
+    asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];"
+                 :: "r"(smem_addr(dst)), "l"(src), "r"(bytes), "r"(smem_addr(bar)) : "memory");
+}
 
 // compile-time loop: f(std::integral_constant<int, I>) for I in [B, E) -- guarantees full unrolling with
 // constant register indices (a plain `#pragma unroll` gave up on the 34 x 8 x 5 nest and spilled to indexing)
@@ -108,10 +139,12 @@ __device__ __forceinline__ void static_for(F&& f) {
     }
 }
 
-// DISC: consecutive tiles overlap by two outputs (tile stride PT_TO - 2, even so that tile origins keep their
-// parity): slot 0 is the output just before the tile's first discriminator output, slot PT_TO-1 is unused.
+// DISC: consecutive tiles overlap by DISC_OV = 4 outputs (tile stride PT_TO - 4): slot 3 is the output just before the
+// tile's first discriminator output (slots 0-2 are unused), and slots 4 .. PT_TO-1 start on 16-byte boundaries of the
+// output whenever tile 0's slot 4 does, so interior tiles store whole float4s.
+constexpr int DISC_OV = 4;
 template <bool DISC>
-struct TileStride { static constexpr int TS = DISC ? PT_TO - 2 : PT_TO; };
+struct TileStride { static constexpr int TS = DISC ? PT_TO - DISC_OV : PT_TO; };
 
 // REAL: real input, real taps, real output (the audio low-pass + de-emphasis + Downsampler(5) stage of the chain,
 // firfilter.lua:147-163 behind the noble identity, see graph.cu).  The two lanes of every float2 register are two
@@ -148,14 +181,54 @@ polyphase_crcf_kernel(const float2* __restrict__ x, const float2* __restrict__ h
     // tile-relative phasors of this thread's first sample pair, E[2 tid] and E[2 tid + 1]; the pair of staging
     // iteration `it` is 2*PT_THREADS*it samples later: E[2u] = A0 * step[it].  (A phasor TABLE in global memory
     // cost one more load stream whose latency was exposed three times per tile -- 42 % of all stall samples.)
+    // BULK: interior tiles of complex data are copied global -> shared by the copy engine (one cp.async.bulk per tile into
+    // the RAW buffer), then rotated into the padded layout.  The copy of a CTA's next tile is issued as soon as the rotation
+    // pass has read the current one, so it has the whole compute phase to land.  No staging registers and no per-thread
+    // global address arithmetic.  (One copy per padded segment instead costs a 68-iteration issue loop per tile: the copy
+    // instruction takes its operands from uniform registers.)
+    // Only the discriminator variant takes this path: it doubles the shared memory of a CTA (5 instead of 8 CTAs per SM),
+    // which made the translator-only tuner (closer to the HBM bound) 13 % slower on H100.
+    constexpr bool BULK = !EDGE && !REAL && DISC;
+    __shared__ __align__(8) uint64_t s_bar;
+    uint32_t bar_phase = 0;
+
     float2 A0 = make_float2(1.f, 0.f), A1 = make_float2(1.f, 0.f);
-    if constexpr (ROT) {
+    // BULK && ROT: thread (g, w) = (tid / PPS, tid % PPS) rotates sample pair w of segments g + RG*it, samples
+    // e = (g + RG*it)*RD + 2w and e + 1.  Their tile-relative phasors E[e] are the same for every tile: they are computed
+    // once, and E[e + 1] = E[e] * W1 costs one complex multiply instead of two (A0 * step[it], A1 * step[it]).
+    const int rg = tid / S::PPS, rw = tid - rg * S::PPS;
+    constexpr int NE0 = (BULK && ROT) ? S::RITERS : 1;
+    float2 E0[NE0];
+    float2 W1 = make_float2(1.f, 0.f);
+    if constexpr (BULK && ROT) {
+        W1 = phasor_from_fix(P.turns_fix);
+#pragma unroll
+        for (int it = 0; it < NE0; ++it)
+            E0[it] = phasor_from_fix(P.turns_fix * (uint64_t)((rg + S::RG * it) * S::RD + 2 * rw));
+    } else if constexpr (ROT) {
         A0 = phasor_from_fix(P.turns_fix * (uint64_t)(2 * tid));
         A1 = phasor_from_fix(P.turns_fix * (uint64_t)(2 * tid + 1));
     }
+    // the last pass reaches past the tile's LOADED samples for some threads
+    const bool rot_last = rg < S::RG && (rg + S::RG * (S::RITERS - 1)) * S::RD + 2 * rw < S::LOADED;
     auto tile_of = [&](long long idx) -> long long { return EDGE ? (idx < t_lo ? idx : t_hi + (idx - t_lo)) : (t_lo + idx); };
     const long long n_work = EDGE ? 0 : (t_hi - t_lo);
     long long widx = blockIdx.x;
+
+    // thread 0 requests tile `idx` of this launch's interior range into RAW.  Callers have passed a barrier behind the
+    // last read of RAW.
+    auto issue_tile = [&](long long idx) {
+        if (tid == 0) {
+            fence_proxy_async();
+            mbar_expect_tx(&s_bar, (uint32_t)(S::LOADED * sizeof(float2)));
+            bulk_g2s(smem + S::RAW, x + (P.off + tile_of(idx) * (long long)(TS * D)), (uint32_t)(S::LOADED * sizeof(float2)), &s_bar);
+        }
+    };
+    if constexpr (BULK) {
+        if (tid == 0) mbar_init(&s_bar);
+        __syncthreads();
+        if (widx < n_work) issue_tile(widx);
+    }
 
     // staging addresses: pair u = tid + 128*it holds samples e = 2u, 2u+1 -> padded element 2u + 2*floor(2u / RD)
     // (RD is even, so a pair never straddles a padding gap and stays 16-byte aligned)
@@ -175,7 +248,7 @@ polyphase_crcf_kernel(const float2* __restrict__ x, const float2* __restrict__ h
     // 44 % of the stall samples sat in the staging / epilogue regions, mostly long-scoreboard waits on these loads)
     constexpr int REST = (S::ITERS - NPRE) < PT_BATCH ? (S::ITERS - NPRE) : PT_BATCH;
     float4 rest[REST > 0 ? REST : 1];
-    if constexpr (!EDGE) {
+    if constexpr (!EDGE && !BULK) {
         if (widx < n_work) {
             const long long Bt = P.off + tile_of(widx) * (long long)(TS * D);
 #pragma unroll
@@ -191,7 +264,7 @@ polyphase_crcf_kernel(const float2* __restrict__ x, const float2* __restrict__ h
         if constexpr (!EDGE) { if (widx >= n_work) break; }
         const long long tile = tile_of(widx);
         const long long B = P.off + tile * (long long)(TS * D);      // first input index of the tile (even)
-        const long long m0 = tile * TS - (DISC ? 1 : 0) - PW;        // output index of slot 0
+        const long long m0 = tile * TS - (DISC ? DISC_OV : 0) - PW;  // output index of slot 0
 
         // ---- stage: global -> (x E) -> shared, natural order
         auto stage_pair = [&](float4 v, int it) {
@@ -204,7 +277,27 @@ polyphase_crcf_kernel(const float2* __restrict__ x, const float2* __restrict__ h
             }
             *reinterpret_cast<float4*>(smem + S::pad(2 * u)) = make_float4(a.x, a.y, b.x, b.y);
         };
-        if constexpr (!EDGE && LRB_PT_EXPERIMENT == 1) {
+        if constexpr (BULK) {
+            if (LRB_PT_EXPERIMENT != 1 || widx == blockIdx.x) {
+                mbar_wait(&s_bar, bar_phase);
+                bar_phase ^= 1;
+                if (rg < S::RG) {
+                    const float2* src = smem + S::RAW + rg * S::RD + 2 * rw;
+                    float2* dst = smem + rg * (S::RD + 2) + 2 * rw;
+#pragma unroll
+                    for (int it = 0; it < S::RITERS; ++it) {
+                        if (it == S::RITERS - 1 && !rot_last) break;
+                        float4 v = *reinterpret_cast<const float4*>(src + it * S::RG * S::RD);
+                        if constexpr (ROT) {
+                            const float2 a = cmul(make_float2(v.x, v.y), E0[it]);
+                            const float2 b = cmul(make_float2(v.z, v.w), cmul(E0[it], W1));
+                            v = make_float4(a.x, a.y, b.x, b.y);
+                        }
+                        *reinterpret_cast<float4*>(dst + it * S::RG * (S::RD + 2)) = v;
+                    }
+                }
+            }
+        } else if constexpr (!EDGE && LRB_PT_EXPERIMENT == 1) {
             if (widx == blockIdx.x) {
 #pragma unroll 1
                 for (int it = 0; it < S::ITERS; ++it) stage_pair(ld_pair(B, it), it);
@@ -251,8 +344,12 @@ polyphase_crcf_kernel(const float2* __restrict__ x, const float2* __restrict__ h
         }
         __syncthreads();
 
+        // BULK: RAW has been read; the next tile's copy lands during the compute phase
+        if constexpr (BULK && LRB_PT_EXPERIMENT != 1) {
+            if (widx + gridDim.x < n_work) issue_tile(widx + gridDim.x);
+        }
         // ---- prefetch the first batch of this CTA's next tile; it stays in registers across the compute phase
-        if constexpr (!EDGE && LRB_PT_EXPERIMENT != 1) {
+        if constexpr (!EDGE && !BULK && LRB_PT_EXPERIMENT != 1) {
             const long long nidx = widx + gridDim.x;
             if (nidx < n_work) {
                 const long long Bn = P.off + tile_of(nidx) * (long long)(TS * D);
@@ -302,7 +399,7 @@ polyphase_crcf_kernel(const float2* __restrict__ x, const float2* __restrict__ h
                 }
             });
         });
-        if constexpr (!EDGE && LRB_PT_EARLY_REST) {
+        if constexpr (!EDGE && !BULK && LRB_PT_EARLY_REST) {
             const long long nidx = widx + gridDim.x;
             if (nidx < n_work) {
                 const long long Bn = P.off + tile_of(nidx) * (long long)(TS * D);
@@ -396,7 +493,7 @@ polyphase_crcf_kernel(const float2* __restrict__ x, const float2* __restrict__ h
             __syncthreads();                               // shared tile is reused by the next iteration
         } else {
             // ---- fused FrequencyDiscriminator (frequencydiscriminator.lua:68-88):
-            //      d[m] = atan2(im, re of y[m] * conj(y[m-1])) * (1/gain); slot 0 only supplies y[m-1] for slot 1
+            //      d[m] = atan2(im, re of y[m] * conj(y[m-1])) * (1/gain); slot DISC_OV-1 only supplies y[m-1] for slot DISC_OV
             float* yd = reinterpret_cast<float*>(yv);
             float2 left;                                   // y just before acc[0]
             left.x = __shfl_up_sync(0xffffffffu, acc[PT_R - 1].x, 1);
@@ -405,18 +502,16 @@ polyphase_crcf_kernel(const float2* __restrict__ x, const float2* __restrict__ h
             __syncthreads();                               // also fences the shared tile for the next iteration
             if (lane == 0 && warp > 0) left = s_edge[warp - 1];
             bool zero_prev = false;                        // the carried sample is exactly (0, 0): stream start
-            if (tid == 0 && tile == 0) {
+            // the stream's first tile and the call's last output are edge work: the launcher never gives them to the interior
+            if (EDGE && tid == 0 && tile == 0) {
                 // stream state: the previous call's last output (absolute phase) brought into this tile's frame
                 const float2 Pt = ROT ? phasor_from_fix(P.turns_fix * (P.g0 + (uint64_t)B)) : make_float2(1.f, 0.f);
                 const float2 pv = __ldg(prev_in);
-                acc[0] = cmul(pv, make_float2(Pt.x, -Pt.y));
-                if constexpr (EDGE) zero_prev = pv.x == 0.f && pv.y == 0.f;   // tile 0 reaches into the history: always an edge tile
+                acc[DISC_OV - 1] = cmul(pv, make_float2(Pt.x, -Pt.y));
+                zero_prev = pv.x == 0.f && pv.y == 0.f;
             }
-            // slots are tile-relative 32-bit indices: slot s holds y[m0 + s]; slots 1 .. lim-1 produce outputs
-            const long long room = n_out - m0;             // > 1 for every launched tile
-            const int lim = room < (long long)(TS + 1) ? (int)room : TS + 1;
             const int s0 = tid * PT_R;
-            float* yt = yd + m0;
+            float* yt = yd + m0;                           // slot s holds y[m0 + s]
             // y[m] * conj(y[m-1]) for the 8 slots, two at a time on packed lanes
             float dout[PT_R];
 #pragma unroll
@@ -437,20 +532,38 @@ polyphase_crcf_kernel(const float2* __restrict__ x, const float2* __restrict__ h
                 // pi / gain at the start of one stream in four.  The packed fast atan2 above works in the tile's rotated
                 // frame and tests x < 0, so this one sample is redone in the absolute frame with IEEE operations.
                 const float2 Pt = ROT ? phasor_from_fix(P.turns_fix * (P.g0 + (uint64_t)B)) : make_float2(1.f, 0.f);
-                const float2 ya = ROT ? cmul(acc[1], Pt) : acc[1];
+                const float2 ya = ROT ? cmul(acc[DISC_OV], Pt) : acc[DISC_OV];
                 const float pz = 0.f, nz = -0.f;
                 const float re = __fsub_rn(__fmul_rn(ya.x, pz), __fmul_rn(ya.y, nz));
                 const float im = __fadd_rn(__fmul_rn(ya.x, nz), __fmul_rn(ya.y, pz));
-                dout[1] = atan2f(im, re) * inv_gain;
+                dout[DISC_OV] = atan2f(im, re) * inv_gain;
             }
+            if constexpr (!EDGE) {
+                // a whole interior tile: slots DISC_OV .. PT_TO-1, 16-byte aligned together with the output's start
+                if (((reinterpret_cast<uintptr_t>(yt) + DISC_OV * sizeof(float)) & 15) == 0) {
+                    static_assert(DISC_OV == 4 && PT_R % 4 == 0, "thread 0 skips exactly its first float4");
 #pragma unroll
-            for (int r = 0; r < PT_R; ++r) {
-                const int sl = s0 + r;
-                if (sl >= 1 && sl < lim) {
-                    yt[sl] = dout[r];
-                    if ((long long)sl == room - 1) {        // last output of the call: carried to the next one, in absolute phase
-                        const float2 Pt = ROT ? phasor_from_fix(P.turns_fix * (P.g0 + (uint64_t)B)) : make_float2(1.f, 0.f);
-                        *prev_out = cmul(acc[r], Pt);
+                    for (int r = 0; r < PT_R; r += 4)
+                        if (tid > 0 || r >= DISC_OV)
+                            *reinterpret_cast<float4*>(yt + s0 + r) = make_float4(dout[r], dout[r + 1], dout[r + 2], dout[r + 3]);
+                } else {
+#pragma unroll
+                    for (int r = 0; r < PT_R; ++r)
+                        if (s0 + r >= DISC_OV) yt[s0 + r] = dout[r];
+                }
+            } else {
+                // slots DISC_OV .. lim-1 produce outputs
+                const long long room = n_out - m0;         // > DISC_OV for every launched tile
+                const int lim = room < (long long)PT_TO ? (int)room : PT_TO;
+#pragma unroll
+                for (int r = 0; r < PT_R; ++r) {
+                    const int sl = s0 + r;
+                    if (sl >= DISC_OV && sl < lim) {
+                        yt[sl] = dout[r];
+                        if ((long long)sl == room - 1) {    // last output of the call: carried to the next one, in absolute phase
+                            const float2 Pt = ROT ? phasor_from_fix(P.turns_fix * (P.g0 + (uint64_t)B)) : make_float2(1.f, 0.f);
+                            *prev_out = cmul(acc[r], Pt);
+                        }
                     }
                 }
             }
@@ -473,18 +586,19 @@ int launch_shape(PolyParams P, const float* hr_base, const float2* x, const floa
     int& ctas_per_sm = ctas_dev[ctx().device & (LRB_MAX_DEVICES - 1)];
     auto kern_i = polyphase_crcf_kernel<D, Q, ROT, DISC, false, REAL, POLE>;
     auto kern_e = polyphase_crcf_kernel<D, Q, ROT, DISC, true, REAL, POLE>;
+    constexpr size_t SMEM_I = (!REAL && DISC) ? S::SMEM_BULK : S::SMEM;   // interior kernel: BULK with the discriminator
     if (!configured) {
-        LRB_CHECK(cudaFuncSetAttribute(kern_i, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)S::SMEM));
+        LRB_CHECK(cudaFuncSetAttribute(kern_i, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)SMEM_I));
         LRB_CHECK(cudaFuncSetAttribute(kern_e, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)S::SMEM));
-        LRB_CHECK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&ctas_per_sm, kern_i, PT_THREADS, S::SMEM));
+        LRB_CHECK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&ctas_per_sm, kern_i, PT_THREADS, SMEM_I));
         if (ctas_per_sm < 1) ctas_per_sm = 1;
         configured = true;
     }
     constexpr int PW = POLE ? PT_POLE_WARM : 0;
     constexpr int PAY = PT_TO - PW;
     constexpr int TS = REAL ? 2 * PAY : TileStride<DISC>::TS;
-    // B(tile) = first + m0*D - (Q*D - 1) - shift, m0 = tile*TS - (DISC ? 1 : 0) - PW; shift in {0,1} makes it even
-    long long off = first - (DISC ? D : 0) - (long long)PW * D - (long long)(Q * D - 1);
+    // B(tile) = first + m0*D - (Q*D - 1) - shift, m0 = tile*TS - (DISC ? DISC_OV : 0) - PW; shift in {0,1} makes it even
+    long long off = first - (DISC ? (long long)DISC_OV * D : 0) - (long long)PW * D - (long long)(Q * D - 1);
     const int shift = (int)(((off % 2) + 2) % 2);
     off -= shift;
     P.off = off;
@@ -506,6 +620,11 @@ int launch_shape(PolyParams P, const float* hr_base, const float2* x, const floa
         const long long lim = n - (long long)S::LOADED - off - (REAL ? (long long)PAY * D : 0);
         t_hi = lim < 0 ? 0 : lim / step + 1;
         if (t_hi > tiles) t_hi = tiles;
+        if (DISC) {
+            // the stream state (prev_in / prev_out) is read in tile 0 and written in the last tile: both run as edge tiles
+            if (t_lo < 1) t_lo = 1;
+            if (t_hi > tiles - 1) t_hi = tiles - 1;
+        }
         if (t_lo > t_hi) t_lo = t_hi;
     }
     const long long n_int = t_hi - t_lo, n_edge = tiles - n_int;
@@ -521,7 +640,7 @@ int launch_shape(PolyParams P, const float* hr_base, const float2* x, const floa
         long long grid = (long long)ctx().sm_count * ctas_per_sm - ctx().reserve_ctas;
         if (grid < 1) grid = 1;
         if (grid > n_int) grid = n_int;
-        kern_i<<<(unsigned)grid, PT_THREADS, S::SMEM, s>>>(x, hist, n, y, n_out, P, t_lo, t_hi, prev_in, prev_out, inv_gain);
+        kern_i<<<(unsigned)grid, PT_THREADS, SMEM_I, s>>>(x, hist, n, y, n_out, P, t_lo, t_hi, prev_in, prev_out, inv_gain);
         count_launch();
     }
     side_join(s, side);

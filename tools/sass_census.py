@@ -69,6 +69,15 @@ def main():
             print("hottest loop: %d instructions at 0x%04x-0x%04x, FFMA2+FFMA %d = %.1f %% of its issue slots" %
                   (len(body), ins[j][0], ins[i][0], fma, 100.0 * fma / len(body)))
             print("  loop mix:", ", ".join("%s %d" % kv for kv in h.most_common(14)))
+            # the loop body between its barriers (static counts): for the persistent tile loop that is staging | compute |
+            # epilogue, give or take where the loop's back edge falls
+            cuts = [k for k, (_, x) in enumerate(body) if mnem(x) == "BAR"]
+            for k0, k1 in zip([0] + [c + 1 for c in cuts], cuts + [len(body)]):
+                seg = body[k0:k1]
+                if seg:
+                    hs = collections.Counter(mnem(x) for _, x in seg)
+                    print("  region 0x%04x-0x%04x: %d instructions: %s" % (seg[0][0], seg[-1][0], len(seg),
+                                                                        ", ".join("%s %d" % kv for kv in hs.most_common(10))))
             print("  excerpt (first 48 instructions of the loop body):")
             for a, t in body[:48]:
                 print("    /*%04x*/ %s" % (a, t))
