@@ -207,6 +207,20 @@ lrb200_block_t* lrb200_delay_create(unsigned num_samples, unsigned elem_size, un
 lrb200_block_t* lrb200_psd_create(unsigned num_samples, const float32_t* window, double scale, unsigned logarithmic,
                                   unsigned complex_data, unsigned flags);
 
+/* ---- AGCBlock / PowerSquelchBlock (the reference's "Level Control" blocks) -------------------------------------------
+ * lrb200_agc_create replaces AGCBlock:process_real / process_complex (radio/blocks/signal/agc.lua:72-115):
+ *   P = (1-pa) P + pa |x|^2;  if P >= threshold: g = (1-ga) g + ga (target (1/P)), y = sqrt(g) x;  else y = x (g held)
+ * with pa = 1/(1 + power_tau*rate), ga = 1/(1 + gain_tau*rate) and the dBFS target / threshold linearised as 10^(v/10)
+ * (agc.lua:57-68), all in double; the output is rounded to float32 once.  lrb200_powersquelch_create replaces
+ * PowerSquelchBlock:process_real / process_complex (radio/blocks/signal/powersquelch.lua:43-75): the same power estimator
+ * with alpha = 1/(1 + tau*rate), y = x if P >= threshold else 0.  (The reference's PowerSquelchBlock always uses
+ * tau = 0.001: powersquelch.lua:26 reads an undefined global, so its second argument is ignored -- its callers pass 0.001.)
+ * complex_data != 0: ComplexFloat32, else Float32.  (P, g) start at zero and are carried across calls.  A block-parallel
+ * scan with decoupled look-back: one kernel launch per call of up to 256 Mi samples. */
+lrb200_block_t* lrb200_agc_create(double target_dbfs, double threshold_dbfs, double gain_tau, double power_tau, double rate,
+                                  unsigned complex_data, unsigned flags);
+lrb200_block_t* lrb200_powersquelch_create(double threshold_dbfs, double tau, double rate, unsigned complex_data, unsigned flags);
+
 /* ---- IQFileSource sample formats (the source boundary, SURVEY.md 8f row 1) ------------------------------
  * Replaces the byte-swap + (value - offset) / scale loops of radio/blocks/sources/iqfile.lua:96-108 with the format
  * table of radio/utilities/format_utils.lua:82-97: u8 s8 u16le u16be s16le s16be u32le u32be s32le s32be f32le f32be

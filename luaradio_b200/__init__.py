@@ -24,7 +24,8 @@ from .signal_blocks import (MultiplyConstantBlock, UpsamplerBlock, BandpassFilte
                             FrequencyDiscriminatorBlock, FrequencyTranslatorBlock, GPUBlock,
                             HighpassFilterBlock, HilbertTransformBlock, IIRFilterBlock, LowpassFilterBlock,
                             SinglepoleHighpassFilterBlock, SinglepoleLowpassFilterBlock,
-                            MultiplyBlock, MultiplyConjugateBlock, AddBlock, SubtractBlock, DelayBlock, PLLBlock, GPUMultiBlock)
+                            MultiplyBlock, MultiplyConjugateBlock, AddBlock, SubtractBlock, DelayBlock, PLLBlock, GPUMultiBlock,
+                            AGCBlock, PowerSquelchBlock)
 from .types import ComplexFloat32, Float32, Vector
 from .utilities import filter_utils, spectrum_utils, window_utils
 

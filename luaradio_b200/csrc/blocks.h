@@ -216,6 +216,28 @@ struct InterpFirBlock : Block {       // [MultiplyConstant ->] Upsampler -> FIR(
     void rate(unsigned* up, unsigned* down) const override { *up = (unsigned)L; *down = (unsigned)D; }
 };
 
+// level.cu: AGCBlock (agc = true) and PowerSquelchBlock, one block-parallel scan kernel per call
+constexpr int LEVEL_MAX_TILES = 1 << 17;   // 2048-sample tiles per launch (256 Mi samples)
+struct LevelBlock : Block {
+    bool agc = false, complex_data = false;
+    double pa = 0, ga = 0, T = 0, theta = 0;  // power / gain alphas, linear target and threshold
+    void* d_state[2] = {nullptr, nullptr};    // (P, g) after the last sample, ping-ponged per launch
+    int cur = 0;
+    double* d_pw = nullptr;                   // (1-ga)^k, k <= one tile
+    void* d_ticket = nullptr;                 // tile tickets, counted up across launches from ticket_base
+    unsigned long long ticket_base = 0;
+    void* d_rec = nullptr;                    // per-tile look-back records, 16 bytes per tile and stage
+    size_t rec_bytes() const { return (size_t)16 * (agc ? 2 : 1) * LEVEL_MAX_TILES; }
+    unsigned epoch = 0;
+    LevelBlock(bool agc, double power_alpha, double gain_alpha, double target, double threshold, bool cplx, bool dev);
+    ~LevelBlock() override;
+    int init() override;
+    void reset_host() override;
+    void state_buffers(std::vector<std::pair<void*, size_t>>& segs) override;
+    int run(const void* dx, size_t n, void* dy, size_t* n_out, cudaStream_t s) override;
+    long long memory_in() const override;
+};
+
 }  // namespace lrb
 
 // the opaque public handle

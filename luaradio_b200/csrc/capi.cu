@@ -734,6 +734,36 @@ lrb200_block_t* lrb200_realsink_create(const char* format, unsigned flags) {
     return b ? wrap(b) : nullptr;
 }
 
+// ---- level control -----------------------------------------------------------------------------
+lrb200_block_t* lrb200_agc_create(double target_dbfs, double threshold_dbfs, double gain_tau, double power_tau, double rate,
+                                  unsigned complex_data, unsigned flags) {
+    if (ensure_init() != 0) return nullptr;
+    if (!(rate > 0.0) || !std::isfinite(rate)) { set_error("agc: rate must be positive"); return nullptr; }
+    if (!(gain_tau >= 0.0) || !(power_tau >= 0.0) || !std::isfinite(gain_tau) || !std::isfinite(power_tau)) {
+        set_error("agc: gain_tau and power_tau must be finite and non-negative");
+        return nullptr;
+    }
+    if (!std::isfinite(target_dbfs) || !std::isfinite(threshold_dbfs)) { set_error("agc: target and threshold must be finite"); return nullptr; }
+    // agc.lua:59-67, in the reference's expression order
+    const double power_alpha = 1 / (1 + power_tau * rate);
+    const double gain_alpha = 1 / (1 + gain_tau * rate);
+    const double target = std::pow(10.0, target_dbfs / 10);
+    const double threshold = std::pow(10.0, threshold_dbfs / 10);
+    return wrap(new (std::nothrow) LevelBlock(true, power_alpha, gain_alpha, target, threshold, complex_data != 0,
+                                              (flags & LRB200_DEVICE) != 0));
+}
+
+lrb200_block_t* lrb200_powersquelch_create(double threshold_dbfs, double tau, double rate, unsigned complex_data, unsigned flags) {
+    if (ensure_init() != 0) return nullptr;
+    if (!(rate > 0.0) || !std::isfinite(rate)) { set_error("powersquelch: rate must be positive"); return nullptr; }
+    if (!(tau >= 0.0) || !std::isfinite(tau)) { set_error("powersquelch: tau must be finite and non-negative"); return nullptr; }
+    if (!std::isfinite(threshold_dbfs)) { set_error("powersquelch: threshold must be finite"); return nullptr; }
+    // powersquelch.lua:34-38
+    const double alpha = 1 / (1 + tau * rate);
+    const double threshold = std::pow(10.0, threshold_dbfs / 10);
+    return wrap(new (std::nothrow) LevelBlock(false, alpha, 0.0, 0.0, threshold, complex_data != 0, (flags & LRB200_DEVICE) != 0));
+}
+
 // ---- synthetic sources -------------------------------------------------------------------------
 int lrb200_synth_white_iq(complex_float32_t* dst, uint64_t n0, size_t n, uint32_t seed) {
     if (ensure_init() != 0) return -1;

@@ -472,3 +472,56 @@ class PLLBlock(GPUMultiBlock):
         if self.parallel:
             _lib.check(lib.lrb200_pll_set_mode(h, 1), "pll_set_mode")
         return h
+
+
+# ---------------------------------------------------------------------------------------------
+# Level control (the reference's "Level Control" category)
+# ---------------------------------------------------------------------------------------------
+class AGCBlock(GPUBlock):
+    """agc.lua:41-115: feed-forward automatic gain control towards `target` dBFS, gated by `threshold` dBFS.
+    gain_tau is 0.1 s ("fast"), 3.0 s ("slow") or options["gain_tau"] ("custom"); power_tau is options["power_tau"] or
+    1.0 s."""
+    name = "AGCBlock"
+
+    def instantiate(self, mode=None, target=None, threshold=None, options=None):
+        assert mode is not None, 'Missing argument #1 (mode), can be "fast", "slow", or "custom"'
+        self.mode = mode
+        self.target = -35 if target is None else target
+        self.threshold = -75 if threshold is None else threshold
+        self.options = options or {}
+        gain_tau = {"fast": 0.1, "slow": 3.0}.get(mode) if isinstance(mode, str) else None
+        self.gain_tau = gain_tau if gain_tau is not None else self.options.get("gain_tau")
+        power_tau = self.options.get("power_tau")
+        self.power_tau = 1.0 if power_tau is None else power_tau
+        assert mode in ("fast", "slow", "custom"), 'Invalid mode "%s"' % (mode,)
+        assert self.gain_tau is not None, 'Missing gain_tau parameter for "custom" mode'
+        self.add_type_signature([Input("in", Float32)], [Output("out", Float32)])
+        self.add_type_signature([Input("in", ComplexFloat32)], [Output("out", ComplexFloat32)])
+
+    def _make_handle(self, flags):
+        cdata = 1 if self.get_input_type() is ComplexFloat32 else 0
+        return _lib.check_handle(_lib.load().lrb200_agc_create(float(self.target), float(self.threshold), float(self.gain_tau),
+                                                               float(self.power_tau), float(self.get_rate()), cdata, flags),
+                                 "lrb200 agc object")
+
+
+class PowerSquelchBlock(GPUBlock):
+    """powersquelch.lua:24-75: y = x while the average power is at least `threshold` dBFS, else 0.
+
+    The power estimator's time constant is always 0.001 s: the reference's instantiate assigns `tau or 0.001` from an
+    undefined global `tau` (powersquelch.lua:26), so its second argument is accepted and ignored.  This block does the
+    same, because the reference's outputs are the contract."""
+    name = "PowerSquelchBlock"
+
+    def instantiate(self, threshold=None, cutoff=None):
+        assert threshold is not None, "Missing argument #1 (threshold)"
+        self.threshold = threshold
+        self.tau = 0.001
+        self.add_type_signature([Input("in", Float32)], [Output("out", Float32)])
+        self.add_type_signature([Input("in", ComplexFloat32)], [Output("out", ComplexFloat32)])
+
+    def _make_handle(self, flags):
+        cdata = 1 if self.get_input_type() is ComplexFloat32 else 0
+        return _lib.check_handle(_lib.load().lrb200_powersquelch_create(float(self.threshold), float(self.tau), float(self.get_rate()),
+                                                                        cdata, flags),
+                                 "lrb200 powersquelch object")

@@ -1,9 +1,9 @@
 #!/usr/bin/env python3
 """Device-side throughput of the kernels on the rows next to the hot path (SURVEY.md 8f): file sample-format converters
-at the graph boundaries and the resampling family.  One JSON object; achieved GB/s counts ALGORITHMIC bytes (input +
+at the graph boundaries, the resampling family and level control (AGCBlock, PowerSquelchBlock, the rx_am envelope chain).  One JSON object; achieved GB/s counts ALGORITHMIC bytes (input +
 output of the block), against the measured HBM peak (MEASURED_PEAKS.json, see bench.peaks()).
 
-    python tools/aux_bench.py [--samples N] [--steps K] > profiles/rNN_aux_bench.json
+    python tools/aux_bench.py [--samples N] [--steps K] [--only-level] > profiles/rNN_aux_bench.json
 """
 import argparse
 import ctypes
@@ -21,6 +21,7 @@ def main():
     ap.add_argument("--samples", type=int, default=1 << 28)
     ap.add_argument("--steps", type=int, default=10)
     ap.add_argument("--only-resample", action="store_true", help="skip the file-format rows")
+    ap.add_argument("--only-level", action="store_true", help="only the level-control rows")
     args = ap.parse_args()
     import torch
     import luaradio_b200 as radio
@@ -67,6 +68,38 @@ def main():
                      "hbm_GBs": round(gbs, 1), "frac_of_peak": round(gbs / peak, 4), "note": note})
         lib.lrb200_graph_destroy(g)
 
+    def timed_calls(name, h, in_ptr, n_in, call, out_ptr, bytes_per_in, note=""):
+        """One block handle (DEVICE pointers) fed `call` samples per execute, state carried: the reference's per-vector
+        regime.  A step is n_in samples in n_in / call launches."""
+        no = ctypes.c_size_t(0)
+        h = _lib.check_handle(h, name)
+        es = bytes_per_in // 2                       # element size: input and output have the same type
+
+        def step():
+            for k in range(0, n_in, call):
+                _lib.check(lib.lrb200_block_execute(h, ctypes.c_void_p(in_ptr + k * es), min(call, n_in - k),
+                                                    ctypes.c_void_p(out_ptr + k * es), ctypes.byref(no)), name)
+
+        step()
+        torch.cuda.synchronize()
+        e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+        e0.record(stream)
+        for _ in range(args.steps):
+            step()
+        e1.record(stream)
+        torch.cuda.synchronize()
+        ms = e0.elapsed_time(e1) / args.steps
+        gbs = bytes_per_in * n_in / (ms * 1e-3) / 1e9
+        rows.append({"kernel": name, "graph": lib.lrb200_block_name(h).decode(), "input_samples": n_in, "samples_per_call": call,
+                     "ms": round(ms, 4), "msamples_per_s": round(n_in / ms / 1e3, 1), "algorithmic_bytes_per_input_sample": bytes_per_in,
+                     "hbm_GBs": round(gbs, 1), "frac_of_peak": round(gbs / peak, 4), "note": note})
+        lib.lrb200_block_destroy(h)
+
+    if args.only_level:
+        level_rows(lib, _lib, radio, timed, timed_calls, x, y, n)
+        print(json.dumps({"peak_GBs": peak, "peak_source": src, "samples": n, "steps": args.steps, "rows": rows}))
+        return
+
     # ---- file formats: fill `raw` with the sink's own output so the source converters read realistic bytes
     for fmt, b in (() if args.only_resample else (("u8", 1), ("s16le", 2), ("f32be", 4))):
         timed("iqsink(%s)" % fmt, lambda: [lib.lrb200_iqsink_create(fmt.encode(), D)], xs.data_ptr(), n, raw.data_ptr(), 8 + 2 * b)
@@ -87,7 +120,43 @@ def main():
             return hs
         timed("interpolator x%d" % L if Dn == 1 else "rational resampler %d/%d" % (L, Dn), make, x.data_ptr(), m, y.data_ptr(),
               8 + 8.0 * L / Dn, "128 taps, complex")
+    level_rows(lib, _lib, radio, timed, timed_calls, x, y, n)
     print(json.dumps({"peak_GBs": peak, "peak_source": src, "samples": n, "steps": args.steps, "rows": rows}))
+
+
+def level_rows(lib, _lib, radio, timed, timed_calls, x, y, n):
+    """AGCBlock('slow') and PowerSquelchBlock(-40) at 1 MS/s on white noise (the gate open throughout: the costly case), the
+    AGC once more with the gate closed throughout (the copy), each as one call of n samples and as 8192-sample calls, and
+    the rx_am envelope chain (rx_am.lua:51-55) at 1.1025 MS/s.  Real rows read the I/Q words as n Float32 samples."""
+    from luaradio_b200.types import ComplexFloat32
+    D = _lib.LRB200_DEVICE
+    for cplx, bpi in ((0, 8), (1, 16)):
+        kind = "complex" if cplx else "real"
+        for label, mk in (("agc(slow) %s" % kind, lambda: lib.lrb200_agc_create(-35.0, -75.0, 3.0, 1.0, 1e6, cplx, D)),
+                          ("agc(slow) %s, gate closed" % kind, lambda: lib.lrb200_agc_create(-35.0, 30.0, 3.0, 1.0, 1e6, cplx, D)),
+                          ("powersquelch(-40) %s" % kind, lambda: lib.lrb200_powersquelch_create(-40.0, 0.001, 1e6, cplx, D))):
+            timed(label, lambda: [mk()], x.data_ptr(), n, y.data_ptr(), bpi, "one call")
+            timed_calls(label + ", 8192-sample calls", mk(), x.data_ptr(), n // 16, 8192, y.data_ptr(), bpi,
+                        "the reference's vector size, one launch per call")
+    rate = 1102500.0
+
+    def dev(blk, in_type, r):
+        blk.get_rate = lambda: r
+        blk.differentiate([in_type])
+        blk.initialize()
+        h = blk.make_device_handle()
+        blk.cleanup()
+        return h
+
+    def envelope_chain():
+        from luaradio_b200.types import Float32
+        af = rate / 25
+        return [dev(radio.FrequencyTranslatorBlock(-50e3), ComplexFloat32, rate), dev(radio.LowpassFilterBlock(128, 5e3), ComplexFloat32, rate),
+                dev(radio.DownsamplerBlock(25), ComplexFloat32, rate), dev(radio.ComplexMagnitudeBlock(), ComplexFloat32, af),
+                dev(radio.SinglepoleHighpassFilterBlock(100), Float32, af), dev(radio.LowpassFilterBlock(128, 5e3), Float32, af),
+                dev(radio.AGCBlock("slow"), Float32, af)]
+    timed("rx_am envelope chain", envelope_chain, x.data_ptr(), n, y.data_ptr(), 8 + 4.0 / 25,
+          "Tuner(-50e3, 10e3, 25) -> AMEnvelopeDemodulator(5e3) -> AGCBlock('slow'); bytes = chain input + output")
 
 
 if __name__ == "__main__":
