@@ -58,6 +58,11 @@ namespace {
 #define LRB_PT_PREFETCH 9
 #define LRB_PT_BATCH 7
 #endif
+#ifndef LRB_PT_CTAS_BULK
+// the bulk-copy interior kernel: its shared memory (44 KB per CTA) allows 5 CTAs per SM, so its register cap is set for
+// 5 rather than 8 (168 registers instead of 128: 10 warps spread over the SM's four 16 K-register partitions)
+#define LRB_PT_CTAS_BULK 5
+#endif
 #ifndef LRB_PT_EXPERIMENT
 #define LRB_PT_EXPERIMENT 0      // timing experiments only: 1 = stage the first tile only, 2 = skip the MAC loop
 #endif
@@ -73,6 +78,7 @@ constexpr int PT_BATCH = LRB_PT_BATCH;       // 128-bit loads issued back to bac
 constexpr int PT_MAXIT = 48;                 // staging iterations (pairs per thread) upper bound
 struct PolyParams {
     float hr[PT_MAXTAPS];        // reversed taps with the launch's alignment shift, zero padded to Q*D + 1
+    float hs[PT_MAXTAPS / 2];    // fast-FIR sum taps: hs[q*D + p] = hr[2q*D + p] + hr[(2q+1)*D + p], q < Q/2 (float32)
     float2 step[PT_MAXIT];       // exp(j*2*pi*turns * 2*PT_THREADS*it): phasor advance of staging iteration `it`
     uint64_t turns_fix;          // turns per sample, 2^-64 units
     uint64_t g0;                 // global index of x[0]
@@ -139,12 +145,15 @@ __device__ __forceinline__ void static_for(F&& f) {
     }
 }
 
-// DISC: consecutive tiles overlap by DISC_OV = 4 outputs (tile stride PT_TO - 4): slot 3 is the output just before the
-// tile's first discriminator output (slots 0-2 are unused), and slots 4 .. PT_TO-1 start on 16-byte boundaries of the
-// output whenever tile 0's slot 4 does, so interior tiles store whole float4s.
+// DISC: consecutive tiles overlap by DISC_OV + DISC_TAIL = 8 outputs (tile stride PT_TO - 8): slot 3 is the output just
+// before the tile's first discriminator output (slots 0-2 are unused), slots 4 .. PT_TO-5 are stored, and they start on
+// 16-byte boundaries of the output whenever tile 0's slot 4 does, so interior tiles store whole float4s.  The last
+// DISC_TAIL slots are not stored: the fast-FIR interior kernel takes one sub-filter of a thread's last output from the
+// next thread, and the tile's last thread has none, so its last output is not computed.
 constexpr int DISC_OV = 4;
+constexpr int DISC_TAIL = 4;
 template <bool DISC>
-struct TileStride { static constexpr int TS = DISC ? PT_TO - DISC_OV : PT_TO; };
+struct TileStride { static constexpr int TS = DISC ? PT_TO - DISC_OV - DISC_TAIL : PT_TO; };
 
 // REAL: real input, real taps, real output (the audio low-pass + de-emphasis + Downsampler(5) stage of the chain,
 // firfilter.lua:147-163 behind the noble identity, see graph.cu).  The two lanes of every float2 register are two
@@ -158,7 +167,7 @@ struct TileStride { static constexpr int TS = DISC ? PT_TO - DISC_OV : PT_TO; };
 // from its predecessor beyond float32 resolution; the stream's very first run takes the carried state instead.  The
 // scan is thread-sequential (R) -> warp Kogge-Stone -> Horner over the 4 warps, both lanes at once on float2 registers.
 template <int D, int Q, bool ROT, bool DISC, bool EDGE, bool REAL = false, bool POLE = false>
-__global__ void __launch_bounds__(PT_THREADS, LRB_PT_CTAS)
+__global__ void __launch_bounds__(PT_THREADS, (!EDGE && !REAL && DISC) ? LRB_PT_CTAS_BULK : LRB_PT_CTAS)
 polyphase_crcf_kernel(const float2* __restrict__ x, const float2* __restrict__ hist, long long n,
                       void* __restrict__ yv, long long n_out, const __grid_constant__ PolyParams P,
                       long long t_lo, long long t_hi,
@@ -189,6 +198,9 @@ polyphase_crcf_kernel(const float2* __restrict__ x, const float2* __restrict__ h
     // Only the discriminator variant takes this path: it doubles the shared memory of a CTA (5 instead of 8 CTAs per SM),
     // which made the translator-only tuner (closer to the HBM bound) 13 % slower on H100.
     constexpr bool BULK = !EDGE && !REAL && DISC;
+    constexpr bool FFA = BULK && LRB_PT_EXPERIMENT != 2;           // fast-FIR compute phase (below)
+    // FFA: per warp, lane 0's A_0 and lane 31's S, B and spare-tap sample of its last output (see the epilogue)
+    __shared__ float2 s_ffa[FFA ? 4 : 1][PT_THREADS / 32];
     __shared__ __align__(8) uint64_t s_bar;
     uint32_t bar_phase = 0;
 
@@ -363,10 +375,9 @@ polyphase_crcf_kernel(const float2* __restrict__ x, const float2* __restrict__ h
 #pragma unroll
         for (int r = 0; r < PT_R; ++r) acc[r] = make_float2(0.f, 0.f);
         const float2* tb = smem + tid * (S::RD + 2);
-        static_for<0, (LRB_PT_EXPERIMENT == 2 ? 1 : PT_R + Q)>([&](auto jc) {
+        // block j of this thread: samples X[B + (tid*R + j)*D + p], p < D, at padded offset j*D + p + 2*floor((j*D + p)/RD)
+        auto load_block = [&](auto jc, float2 (&xs)[D]) {
             constexpr int j = decltype(jc)::value;
-            // samples X[B + (tid*R + j)*D + p], p < D: padded offset j*D + p + 2*floor((j*D + p)/RD)
-            float2 xs[D];
             constexpr int e0 = j * D;
             if constexpr (j == PT_R + Q - 1) {
                 xs[0] = tb[S::pad(e0)];                            // the last position only feeds tap Q*D (p = 0)
@@ -385,20 +396,114 @@ polyphase_crcf_kernel(const float2* __restrict__ x, const float2* __restrict__ h
                     }
                 });
             }
-            static_for<0, PT_R>([&](auto rc) {
-                constexpr int r = decltype(rc)::value;
-                constexpr int qq = j - r;
-                if constexpr (qq >= 0 && qq <= Q) {
-                    static_for<0, D>([&](auto pc) {
-                        constexpr int pp = decltype(pc)::value;
-                        if constexpr (qq * D + pp < S::T) {
-                            const float h = P.hr[qq * D + pp];
-                            acc[r] = ffma2(xs[pp], make_float2(h, h), acc[r]);
+        };
+        // BULK: two-parallel fast FIR.  With blocks u_j (D samples each) and the tap blocks g_q = hr[qD .. qD+D), split
+        // into even and odd tap blocks G0_q = g_2q, G1_q = g_2q+1 (q < Q/2), each output pair (2k, 2k+1) is
+        //     y[2k]   = A_k + B_k,       y[2k+1] = S_k - A_{k+1} - B_k,
+        //     A_k = sum_q <G0_q, u_2(k+q)>,   B_k = sum_q <G1_q, u_2(k+q)+1>,   S_k = sum_q <G0_q + G1_q, V_k+q>,
+        // with V_i = u_2i+1 + u_2i+2 formed in registers (the odd block is kept until the next even one is loaded) and
+        // G0 + G1 summed on the host (P.hs).  A thread's A_{R/2} is the next thread's A_0 (its blocks start R blocks
+        // later), summed in the same order, so it is taken from there: by shuffle within a warp, through shared memory
+        // across warps in the epilogue; the tile's last thread has no next thread, and its last output is one of the
+        // DISC_TAIL slots that are not stored.  12 sub-filters of Q/2 blocks for the R = 8 outputs instead of 8 filters
+        // of Q blocks: 1576 FFMA per thread and tile (spare tap included) instead of 2096, plus 80 complex adds for V.
+        // The spare tap hr[Q*D] (block Q, p = 0) stays direct.  Output r is formed at block j = Q + r, the one that holds
+        // its spare-tap sample: by then every sub-filter it needs is complete, so they retire as the walk goes on.
+        float2 ffa_a0, ffa_fs, ffa_fb, ffa_sp;           // FFA: what the epilogue's exchange of the last output needs
+        const float hq = P.hr[Q * D];
+        if constexpr (FFA) {
+            static_assert(Q % 2 == 0 && PT_R % 2 == 0 && (Q / 2) * D <= PT_MAXTAPS / 2, "fast-FIR split needs even Q and R");
+            static_assert(DISC_TAIL >= 1, "the tile's last output has no A_{R/2}");
+            constexpr int QH = Q / 2, KP = PT_R / 2;
+            float2 fa[KP], fb[KP], fs[KP], uo[D], an;
+#pragma unroll
+            for (int k = 0; k < KP; ++k) fa[k] = fb[k] = fs[k] = make_float2(0.f, 0.f);
+            static_for<0, PT_R + Q>([&](auto jc) {
+                constexpr int j = decltype(jc)::value;
+                float2 xs[D];
+                load_block(jc, xs);
+                if constexpr (j == PT_R + Q - 1) {
+                    // only the spare tap reads this block
+                } else if constexpr (j % 2 == 0) {
+                    constexpr int i = j / 2;
+                    static_for<0, KP>([&](auto kc) {              // u_2i feeds A_k, q = i - k
+                        constexpr int k = decltype(kc)::value, q = i - k;
+                        if constexpr (q >= 0 && q < QH) {
+                            static_for<0, D>([&](auto pc) {
+                                constexpr int pp = decltype(pc)::value;
+                                const float h = P.hr[2 * q * D + pp];
+                                fa[k] = ffma2(xs[pp], make_float2(h, h), fa[k]);
+                            });
                         }
                     });
+                    if constexpr (i >= 1 && i - 1 <= KP - 1 + QH - 1) {
+                        float2 v[D];                               // V_{i-1} = u_2i-1 + u_2i feeds S_k, q = i - 1 - k
+#pragma unroll
+                        for (int pp = 0; pp < D; ++pp) v[pp] = fadd2(uo[pp], xs[pp]);
+                        static_for<0, KP>([&](auto kc) {
+                            constexpr int k = decltype(kc)::value, q = i - 1 - k;
+                            if constexpr (q >= 0 && q < QH) {
+                                static_for<0, D>([&](auto pc) {
+                                    constexpr int pp = decltype(pc)::value;
+                                    const float h = P.hs[q * D + pp];
+                                    fs[k] = ffma2(v[pp], make_float2(h, h), fs[k]);
+                                });
+                            }
+                        });
+                    }
+                } else {
+                    constexpr int i = (j - 1) / 2;
+                    static_for<0, KP>([&](auto kc) {              // u_2i+1 feeds B_k, q = i - k
+                        constexpr int k = decltype(kc)::value, q = i - k;
+                        if constexpr (q >= 0 && q < QH) {
+                            static_for<0, D>([&](auto pc) {
+                                constexpr int pp = decltype(pc)::value;
+                                const float h = P.hr[(2 * q + 1) * D + pp];
+                                fb[k] = ffma2(xs[pp], make_float2(h, h), fb[k]);
+                            });
+                        }
+                    });
+#pragma unroll
+                    for (int pp = 0; pp < D; ++pp) uo[pp] = xs[pp];
+                }
+                if constexpr (j == 2 * QH - 1) {
+                    // A_0 is complete (its last block was 2 QH - 2): the next lane's is this thread's A_{R/2}
+                    an = make_float2(__shfl_down_sync(0xffffffffu, fa[0].x, 1), __shfl_down_sync(0xffffffffu, fa[0].y, 1));
+                }
+                if constexpr (j >= Q) {
+                    // A_k, B_k are complete from block 2k + Q - 1 on; S_k and A_{k+1} from block 2k + Q
+                    constexpr int r = j - Q, k = r / 2;
+                    if constexpr (r % 2 == 0) {
+                        acc[r] = ffma2(xs[0], make_float2(hq, hq), fadd2(fa[k], fb[k]));
+                    } else if constexpr (k + 1 < KP) {
+                        acc[r] = ffma2(xs[0], make_float2(hq, hq), fsub2(fsub2(fs[k], fa[k + 1]), fb[k]));
+                    } else {
+                        // lane 31's `an` is its own A_0, not its A_{R/2}: the epilogue redoes that lane's last output
+                        acc[r] = ffma2(xs[0], make_float2(hq, hq), fsub2(fsub2(fs[k], an), fb[k]));
+                        ffa_a0 = fa[0]; ffa_fs = fs[k]; ffa_fb = fb[k]; ffa_sp = xs[0];
+                    }
                 }
             });
-        });
+        } else {
+            static_for<0, (LRB_PT_EXPERIMENT == 2 ? 1 : PT_R + Q)>([&](auto jc) {
+                constexpr int j = decltype(jc)::value;
+                float2 xs[D];
+                load_block(jc, xs);
+                static_for<0, PT_R>([&](auto rc) {
+                    constexpr int r = decltype(rc)::value;
+                    constexpr int qq = j - r;
+                    if constexpr (qq >= 0 && qq <= Q) {
+                        static_for<0, D>([&](auto pc) {
+                            constexpr int pp = decltype(pc)::value;
+                            if constexpr (qq * D + pp < S::T) {
+                                const float h = P.hr[qq * D + pp];
+                                acc[r] = ffma2(xs[pp], make_float2(h, h), acc[r]);
+                            }
+                        });
+                    }
+                });
+            });
+        }
         if constexpr (!EDGE && !BULK && LRB_PT_EARLY_REST) {
             const long long nidx = widx + gridDim.x;
             if (nidx < n_work) {
@@ -498,9 +603,24 @@ polyphase_crcf_kernel(const float2* __restrict__ x, const float2* __restrict__ h
             float2 left;                                   // y just before acc[0]
             left.x = __shfl_up_sync(0xffffffffu, acc[PT_R - 1].x, 1);
             left.y = __shfl_up_sync(0xffffffffu, acc[PT_R - 1].y, 1);
-            if (lane == 31) s_edge[warp] = acc[PT_R - 1];
+            if constexpr (FFA) {
+                // lane 31's last output needs the next warp's A_0: lane 0 publishes its A_0 and lane 31 the other terms,
+                // and after the barrier both form that output from the same values in the same order
+                if (lane == 0) s_ffa[0][warp] = ffa_a0;
+                if (lane == 31) { s_ffa[1][warp] = ffa_fs; s_ffa[2][warp] = ffa_fb; s_ffa[3][warp] = ffa_sp; }
+            } else {
+                if (lane == 31) s_edge[warp] = acc[PT_R - 1];
+            }
             __syncthreads();                               // also fences the shared tile for the next iteration
-            if (lane == 0 && warp > 0) left = s_edge[warp - 1];
+            if constexpr (FFA) {
+                auto last_out = [&](int w, float2 a) {
+                    return ffma2(s_ffa[3][w], make_float2(hq, hq), fsub2(fsub2(s_ffa[1][w], a), s_ffa[2][w]));
+                };
+                if (lane == 0 && warp > 0) left = last_out(warp - 1, ffa_a0);
+                if (lane == 31 && warp + 1 < PT_THREADS / 32) acc[PT_R - 1] = last_out(warp, s_ffa[0][warp + 1]);
+            } else {
+                if (lane == 0 && warp > 0) left = s_edge[warp - 1];
+            }
             bool zero_prev = false;                        // the carried sample is exactly (0, 0): stream start
             // the stream's first tile and the call's last output are edge work: the launcher never gives them to the interior
             if (EDGE && tid == 0 && tile == 0) {
@@ -539,22 +659,23 @@ polyphase_crcf_kernel(const float2* __restrict__ x, const float2* __restrict__ h
                 dout[DISC_OV] = atan2f(im, re) * inv_gain;
             }
             if constexpr (!EDGE) {
-                // a whole interior tile: slots DISC_OV .. PT_TO-1, 16-byte aligned together with the output's start
+                // a whole interior tile: slots DISC_OV .. PT_TO-DISC_TAIL-1, 16-byte aligned together with the output's start
                 if (((reinterpret_cast<uintptr_t>(yt) + DISC_OV * sizeof(float)) & 15) == 0) {
-                    static_assert(DISC_OV == 4 && PT_R % 4 == 0, "thread 0 skips exactly its first float4");
+                    static_assert(DISC_OV == 4 && DISC_TAIL == 4 && PT_R % 4 == 0,
+                                  "thread 0 skips exactly its first float4, the last thread exactly its last");
 #pragma unroll
                     for (int r = 0; r < PT_R; r += 4)
-                        if (tid > 0 || r >= DISC_OV)
+                        if ((tid > 0 || r >= DISC_OV) && (tid < PT_THREADS - 1 || r < PT_R - DISC_TAIL))
                             *reinterpret_cast<float4*>(yt + s0 + r) = make_float4(dout[r], dout[r + 1], dout[r + 2], dout[r + 3]);
                 } else {
 #pragma unroll
                     for (int r = 0; r < PT_R; ++r)
-                        if (s0 + r >= DISC_OV) yt[s0 + r] = dout[r];
+                        if (s0 + r >= DISC_OV && s0 + r < PT_TO - DISC_TAIL) yt[s0 + r] = dout[r];
                 }
             } else {
-                // slots DISC_OV .. lim-1 produce outputs
+                // slots DISC_OV .. lim-1 produce outputs (the next tile's slots start at PT_TO - DISC_TAIL)
                 const long long room = n_out - m0;         // > DISC_OV for every launched tile
-                const int lim = room < (long long)PT_TO ? (int)room : PT_TO;
+                const int lim = room < (long long)(PT_TO - DISC_TAIL) ? (int)room : PT_TO - DISC_TAIL;
 #pragma unroll
                 for (int r = 0; r < PT_R; ++r) {
                     const int sl = s0 + r;
@@ -607,6 +728,9 @@ int launch_shape(PolyParams P, const float* hr_base, const float2* x, const floa
         const int k = i - shift;
         P.hr[i] = (k >= 0 && k < Q * D) ? hr_base[k] : 0.0f;
     }
+    // sum taps of the fast-FIR interior kernel, rounded to float32 once here
+    for (int q = 0; 2 * q + 1 < Q; ++q)
+        for (int p = 0; p < D; ++p) P.hs[q * D + p] = P.hr[2 * q * D + p] + P.hr[(2 * q + 1) * D + p];
     const long long tiles = (n_out + TS - 1) / TS;
     // interior tiles: every staged sample B(t) .. B(t)+LOADED-1 inside [lead, n) and x 16-byte aligned (lead > 0: the
     // first samples arrive with the neighbour exchange of a sharded run, see Ctx::lead_samples)
