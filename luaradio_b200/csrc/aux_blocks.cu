@@ -340,11 +340,10 @@ pll_out_kernel(const float* __restrict__ err, long long n, float2* __restrict__ 
 struct PllBlock : Block {
     PllParams P;
     double init_freq;
-    double* d_state = nullptr;      // phi_locked, phi_multiplied, freq_locked, (scratch) phi_multiplied at call start
+    DeviceBuffer d_state;           // phi_locked, phi_multiplied, freq_locked, (scratch) phi_multiplied at call start
     int mode = 0;                   // 0 = exact sequential, 1 = chunk-parallel (locked loop)
     long long warm = 0;             // lead-in of the chunk-parallel form
-    PllChunk* d_chunks = nullptr;
-    int chunk_cap = 0;
+    DeviceBuffer d_chunks;
     PllBlock(double loop_bw_hz, double fmin_hz, double fmax_hz, double multiplier, double rate, bool dev) {
         name = "pll";
         in_size = 8;
@@ -364,21 +363,17 @@ struct PllBlock : Block {
         init_freq = (P.fmin + P.fmax) / 2.0;
         warm = (long long)std::ceil(24.0 / (damping * bw));
     }
-    ~PllBlock() override { cudaFree(d_state); cudaFree(d_chunks); }
     size_t out_size_of(int port) const override { return port == 0 ? 8 : 4; }
     long long memory_in() const override { return -1; }        // the multiplied phase integrates the whole past
-    int set_state(cudaStream_t s) {
+    // the state after create and reset is not zero (freq_locked = init_freq): not carry()-declared
+    int set_state() {
         const double h[3] = {0.0, 0.0, init_freq};
-        LRB_CHECK(cudaMemcpyAsync(d_state, h, sizeof(h), cudaMemcpyHostToDevice, s));
-        return 0;
-    }
-    int init() override {
-        LRB_CHECK(cudaMalloc(&d_state, 4 * sizeof(double)));
-        if (set_state(ctx().stream) != 0) return -1;
+        LRB_CHECK(cudaMemcpyAsync(d_state.get(), h, sizeof(h), cudaMemcpyHostToDevice, ctx().stream));
         LRB_CHECK(cudaStreamSynchronize(ctx().stream));
         return 0;
     }
-    void reset_host() override { consumed = 0; set_state(ctx().stream); cudaStreamSynchronize(ctx().stream); }
+    int init() override { return d_state.reserve(4 * sizeof(double)) != 0 ? -1 : set_state(); }
+    int reset() override { consumed = 0; return set_state(); }
     int run(const void*, size_t, void*, size_t*, cudaStream_t) override {
         set_error("pll has two outputs (out, error): use lrb200_block_execute_multi");
         return -1;
@@ -390,23 +385,22 @@ struct PllBlock : Block {
         const long long L = warm * 4 > 16384 ? warm * 4 : 16384;
         if (mode == 1 && (long long)n >= 2 * L) {
             const int nchunks = (int)(((long long)n + L - 1) / L);
-            if (nchunks > chunk_cap) {
+            if (sizeof(PllChunk) * (size_t)nchunks > d_chunks.capacity()) {
                 LRB_CHECK(cudaStreamSynchronize(s));
-                cudaFree(d_chunks);
-                d_chunks = nullptr;
-                LRB_CHECK(cudaMalloc(&d_chunks, sizeof(PllChunk) * (size_t)nchunks));
-                chunk_cap = nchunks;
+                if (d_chunks.reserve(sizeof(PllChunk) * (size_t)nchunks) != 0) return -1;
             }
             const int blocks = (nchunks + 127) / 128;
-            pll_sim_kernel<<<blocks, 128, 0, s>>>((const float2*)dx[0], (long long)n, (float*)dy[1], L, warm, nchunks, d_state, P, d_chunks);
-            pll_prefix_kernel<<<1, 32, 0, s>>>(d_chunks, nchunks, d_state, P);
-            pll_out_kernel<<<blocks, 128, 0, s>>>((const float*)dy[1], (long long)n, (float2*)dy[0], L, nchunks, d_state, P, d_chunks);
+            PllChunk* chunks = d_chunks.as<PllChunk>();
+            double* st = d_state.as<double>();
+            pll_sim_kernel<<<blocks, 128, 0, s>>>((const float2*)dx[0], (long long)n, (float*)dy[1], L, warm, nchunks, st, P, chunks);
+            pll_prefix_kernel<<<1, 32, 0, s>>>(chunks, nchunks, st, P);
+            pll_out_kernel<<<blocks, 128, 0, s>>>((const float*)dy[1], (long long)n, (float2*)dy[0], L, nchunks, st, P, chunks);
             count_launch(3);
             LRB_CHECK(cudaGetLastError());
             consumed += n;
             return 0;
         }
-        pll_kernel<<<1, 32, 0, s>>>((const float2*)dx[0], (long long)n, (float2*)dy[0], (float*)dy[1], d_state, P);
+        pll_kernel<<<1, 32, 0, s>>>((const float2*)dx[0], (long long)n, (float2*)dy[0], (float*)dy[1], d_state.as<double>(), P);
         count_launch();
         LRB_CHECK(cudaGetLastError());
         consumed += n;
@@ -455,34 +449,22 @@ struct BinaryBlock : Block {
 
 struct DelayBlock : Block {
     long long D;
-    void* d_state[2] = {nullptr, nullptr};
+    DeviceBuffer d_state[2];
     int cur = 0;
     DelayBlock(unsigned num_samples, unsigned elem, bool dev) : D(num_samples) {
         name = "delay";
         in_size = out_size = elem;
         dev_ptrs = dev;
     }
-    ~DelayBlock() override { cudaFree(d_state[0]); cudaFree(d_state[1]); }
-    int init() override {
-        for (int i = 0; i < 2; ++i) {
-            LRB_CHECK(cudaMalloc(&d_state[i], (size_t)D * in_size));
-            LRB_CHECK(cudaMemset(d_state[i], 0, (size_t)D * in_size));
-        }
-        return 0;
-    }
-    void reset_host() override { consumed = 0; cur = 0; }
-    void state_buffers(std::vector<std::pair<void*, size_t>>& segs) override {
-        segs.push_back({d_state[0], (size_t)D * in_size});
-        segs.push_back({d_state[1], (size_t)D * in_size});
-    }
+    int init() override { return carry(d_state, (size_t)D * in_size, cur); }
     long long memory_in() const override { return D; }
     int run(const void* dx, size_t n, void* dy, size_t* n_out, cudaStream_t s) override {
         *n_out = n;
         if (n == 0) return 0;
         const long long wpe = (long long)in_size / 4;
         const long long nw = (long long)n * wpe, Dw = D * wpe;
-        delay_kernel<<<ax_grid(nw > Dw ? nw : Dw), AX_THREADS, 0, s>>>((const uint32_t*)dx, (const uint32_t*)d_state[cur],
-                                                                        (uint32_t*)d_state[cur ^ 1], (uint32_t*)dy, nw, Dw);
+        delay_kernel<<<ax_grid(nw > Dw ? nw : Dw), AX_THREADS, 0, s>>>((const uint32_t*)dx, d_state[cur].as<const uint32_t>(),
+                                                                        d_state[cur ^ 1].as<uint32_t>(), (uint32_t*)dy, nw, Dw);
         count_launch();
         LRB_CHECK(cudaGetLastError());
         cur ^= 1;
@@ -496,9 +478,9 @@ struct PsdBlock : Block {
     bool cplx, logarithmic;
     float inv_scale;
     std::vector<float> h_window;
-    float* d_window = nullptr;
-    float2* d_tw = nullptr;
-    float2* d_tw1024 = nullptr;      // N == 1024: inter-pass twiddles of the register-resident transform
+    DeviceBuffer d_window;
+    DeviceBuffer d_tw;
+    DeviceBuffer d_tw1024;           // N == 1024: inter-pass twiddles of the register-resident transform
     PsdBlock(int N_, const float* window, double scale, bool log_, bool cplx_, bool dev)
         : N(N_), cplx(cplx_), logarithmic(log_), inv_scale((float)(1.0 / scale)) {
         name = "psd";
@@ -509,15 +491,12 @@ struct PsdBlock : Block {
         while ((1 << logN) < N) ++logN;
         h_window.assign(window, window + N);
     }
-    ~PsdBlock() override { cudaFree(d_window); cudaFree(d_tw); cudaFree(d_tw1024); }
     int init() override {
         std::vector<float2> tw((size_t)N / 2 + 1);
         for (int k = 0; k < N / 2; ++k)
             tw[(size_t)k] = make_float2((float)std::cos(2 * M_PI * k / N), (float)(-std::sin(2 * M_PI * k / N)));
-        LRB_CHECK(cudaMalloc(&d_window, sizeof(float) * (size_t)N));
-        LRB_CHECK(cudaMalloc(&d_tw, sizeof(float2) * ((size_t)N / 2 + 1)));
-        LRB_CHECK(cudaMemcpy(d_window, h_window.data(), sizeof(float) * (size_t)N, cudaMemcpyHostToDevice));
-        LRB_CHECK(cudaMemcpy(d_tw, tw.data(), sizeof(float2) * ((size_t)N / 2 + 1), cudaMemcpyHostToDevice));
+        if (d_window.upload(h_window.data(), sizeof(float) * (size_t)N) != 0 || d_tw.upload(tw.data(), sizeof(float2) * tw.size()) != 0)
+            return -1;
         if (N == 1024) {
             std::vector<float2> t2(1024);
             for (int a = 0; a < 32; ++a)
@@ -525,8 +504,7 @@ struct PsdBlock : Block {
                     const int e = (a * c) % 1024;
                     t2[(size_t)a * 32 + c] = make_float2((float)std::cos(2 * M_PI * e / 1024.0), (float)(-std::sin(2 * M_PI * e / 1024.0)));
                 }
-            LRB_CHECK(cudaMalloc(&d_tw1024, sizeof(float2) * 1024));
-            LRB_CHECK(cudaMemcpy(d_tw1024, t2.data(), sizeof(float2) * 1024, cudaMemcpyHostToDevice));
+            if (d_tw1024.upload(t2.data(), sizeof(float2) * t2.size()) != 0) return -1;
         }
         return 0;
     }
@@ -541,15 +519,15 @@ struct PsdBlock : Block {
             long long ctas = ((long long)frames + PS_WARPS - 1) / PS_WARPS;
             const long long cap = (long long)ctx().sm_count * 4;
             if (ctas > cap) ctas = cap;
-            psd1024_kernel<<<(unsigned)ctas, PS_WARPS * 32, smem, s>>>(dx, d_window, (float*)dy, (long long)frames, cplx ? 1 : 0, inv_scale,
-                                                                        logarithmic ? 1 : 0, d_tw1024);
+            psd1024_kernel<<<(unsigned)ctas, PS_WARPS * 32, smem, s>>>(dx, d_window.as<float>(), (float*)dy, (long long)frames, cplx ? 1 : 0, inv_scale,
+                                                                        logarithmic ? 1 : 0, d_tw1024.as<float2>());
             count_launch();
             LRB_CHECK(cudaGetLastError());
             consumed += n;
             return 0;
         }
-        psd_kernel<<<(unsigned)frames, 256, sizeof(float2) * (size_t)N, s>>>(dx, d_window, (float*)dy, N, logN, cplx ? 1 : 0,
-                                                                              inv_scale, logarithmic ? 1 : 0, d_tw);
+        psd_kernel<<<(unsigned)frames, 256, sizeof(float2) * (size_t)N, s>>>(dx, d_window.as<float>(), (float*)dy, N, logN, cplx ? 1 : 0,
+                                                                              inv_scale, logarithmic ? 1 : 0, d_tw.as<float2>());
         count_launch();
         LRB_CHECK(cudaGetLastError());
         consumed += n;
@@ -561,15 +539,6 @@ struct PsdBlock : Block {
 
 using namespace lrb;
 
-template <typename B>
-static lrb200_block_t* wrap_aux(B* b) {
-    if (!b) { set_error("out of memory"); return nullptr; }
-    if (b->init() != 0) { delete b; return nullptr; }
-    lrb200_block_t* h = new (std::nothrow) lrb200_block_s{b};
-    if (!h) { delete b; set_error("out of memory"); }
-    return h;
-}
-
 extern "C" {
 
 lrb200_block_t* lrb200_binary_create(const char* op, unsigned complex_data, unsigned flags) {
@@ -578,7 +547,7 @@ lrb200_block_t* lrb200_binary_create(const char* op, unsigned complex_data, unsi
     int code = o == "multiply" ? BIN_MUL : o == "multiplyconjugate" ? BIN_MULCONJ : o == "add" ? BIN_ADD : o == "subtract" ? BIN_SUB : -1;
     if (code < 0) { set_error("binary: unknown operation \"%s\" (multiply, multiplyconjugate, add, subtract)", o.c_str()); return nullptr; }
     if (code == BIN_MULCONJ && !complex_data) { set_error("binary: multiplyconjugate needs complex data"); return nullptr; }
-    return wrap_aux(new (std::nothrow) BinaryBlock(code, complex_data != 0, (flags & LRB200_DEVICE) != 0));
+    return create_block<BinaryBlock>(flags, code, complex_data != 0);
 }
 
 lrb200_block_t* lrb200_pll_create(double loop_bandwidth, double frequency_min, double frequency_max, double multiplier,
@@ -586,7 +555,7 @@ lrb200_block_t* lrb200_pll_create(double loop_bandwidth, double frequency_min, d
     if (ctx().device < 0 && lrb200_init(0) != 0) return nullptr;
     if (!(rate > 0.0) || !(loop_bandwidth > 0.0) || !std::isfinite(multiplier)) { set_error("pll: rate and loop bandwidth must be positive"); return nullptr; }
     if (!(frequency_min <= frequency_max)) { set_error("pll: frequency_min must not exceed frequency_max"); return nullptr; }
-    return wrap_aux(new (std::nothrow) PllBlock(loop_bandwidth, frequency_min, frequency_max, multiplier, rate, (flags & LRB200_DEVICE) != 0));
+    return create_block<PllBlock>(flags, loop_bandwidth, frequency_min, frequency_max, multiplier, rate);
 }
 
 int lrb200_pll_set_mode(lrb200_block_t* q, int mode) {
@@ -601,7 +570,7 @@ lrb200_block_t* lrb200_delay_create(unsigned num_samples, unsigned elem_size, un
     if (ctx().device < 0 && lrb200_init(0) != 0) return nullptr;
     if (num_samples == 0) { set_error("delay: number of samples must be greater than 0"); return nullptr; }
     if (elem_size != 4 && elem_size != 8) { set_error("delay: elem_size must be 4 or 8"); return nullptr; }
-    return wrap_aux(new (std::nothrow) DelayBlock(num_samples, elem_size, (flags & LRB200_DEVICE) != 0));
+    return create_block<DelayBlock>(flags, num_samples, elem_size);
 }
 
 lrb200_block_t* lrb200_psd_create(unsigned num_samples, const float32_t* window, double scale, unsigned logarithmic,
@@ -613,8 +582,7 @@ lrb200_block_t* lrb200_psd_create(unsigned num_samples, const float32_t* window,
     }
     if (!window) { set_error("psd: missing window"); return nullptr; }
     if (!(scale > 0.0)) { set_error("psd: scale (sample rate * window energy) must be positive"); return nullptr; }
-    return wrap_aux(new (std::nothrow) PsdBlock((int)num_samples, (const float*)window, scale, logarithmic != 0, complex_data != 0,
-                                                (flags & LRB200_DEVICE) != 0));
+    return create_block<PsdBlock>(flags, (int)num_samples, (const float*)window, scale, logarithmic != 0, complex_data != 0);
 }
 
 }  // extern "C"

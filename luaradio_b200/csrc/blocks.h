@@ -1,6 +1,10 @@
 // Block objects behind the opaque C handles (internal).
 #pragma once
+#include "../../include/lrb200.h"
 #include "common.cuh"
+#include <cmath>
+#include <memory>
+#include <new>
 #include <vector>
 #include <string>
 #include <utility>
@@ -12,10 +16,8 @@ struct Block {
     size_t in_size = 8, out_size = 8;
     bool dev_ptrs = false;
     uint64_t consumed = 0;            // global index of the next input sample
-    void* d_in = nullptr;  size_t d_in_cap = 0;    // host-mode staging (grow-only, like Vector:resize)
-    void* d_out = nullptr; size_t d_out_cap = 0;
 
-    virtual ~Block();
+    virtual ~Block() = default;
     virtual int init() { return 0; }
     virtual size_t max_output(size_t n) const { return n; }
     int num_inputs = 1, num_outputs = 1;
@@ -27,14 +29,19 @@ struct Block {
         return run(dx[0], n, dy[0], n_out, s);
     }
     int execute_multi(const void* const* x, int nin, size_t n, void* const* y, int nout, size_t* n_out);
+    int execute(const void* x, size_t n, void* y, size_t* n_out) { return execute_multi(&x, 1, n, &y, 1, n_out); }
     virtual size_t out_size_of(int port) const { (void)port; return out_size; }    // element size of output port `port`
-    std::vector<void*> m_bufs;        // host-mode staging of execute_multi: nin + nout device buffers
-    std::vector<size_t> m_caps;
-    // reset = host-side bookkeeping + zeroing the device state buffers; a graph zeroes every stage's buffers with ONE
-    // kernel (a 256 Mi-sample chain step is ~1 ms: a dozen cudaMemsetAsync nodes per step were 1.5 % of it)
-    virtual void reset_host() { consumed = 0; }
-    virtual void state_buffers(std::vector<std::pair<void*, size_t>>& segs) { (void)segs; }
-    int reset();
+    std::vector<DeviceBuffer> staging;  // host-mode staging of execute_multi: nin + nout grow-only device buffers
+    // Carried state: init() declares each buffer once with carry(), which allocates it zeroed.  reset() zeroes exactly
+    // the declared buffers, puts every ping-pong index back to 0 and sets consumed = 0; a graph zeroes every stage's
+    // buffers with ONE kernel (a 256 Mi-sample chain step is ~1 ms: a dozen cudaMemsetAsync nodes per step were 1.5 % of
+    // it).  Look-back scratch whose counters live on the host is not state and is not declared.
+    std::vector<std::pair<void*, size_t>> carried;
+    std::vector<int*> carried_index;
+    int carry(DeviceBuffer& buf, size_t bytes);
+    int carry(DeviceBuffer (&pair)[2], size_t bytes, int& cur);    // ping-pong pair, buffer `cur` is read
+    void rewind();                    // the host side of reset: indices and consumed
+    virtual int reset();
     virtual int seek(uint64_t idx) { consumed = idx; return 0; }
     // number of outputs this block has produced once `idx` inputs are consumed (for graph seek)
     virtual uint64_t outputs_before(uint64_t idx) const { return idx; }
@@ -50,9 +57,31 @@ struct Block {
     // stream for a long call (edge tiles, history update)?  Then a short call may run entirely on the side stream and the
     // next long call's interior kernel need not wait for it (run_shard's split of the last stage).
     virtual bool state_only_on_side_stream() const { return false; }
-    int execute(const void* x, size_t n, void* y, size_t* n_out);
-    static int reserve(void** p, size_t* cap, size_t bytes);
 };
+
+// Construct and init() a block: nullptr, with the error set, on failure
+template <typename B, typename... A>
+std::unique_ptr<B> make_block(A&&... args) {
+    std::unique_ptr<B> b(new (std::nothrow) B(std::forward<A>(args)...));
+    if (!b) { set_error("out of memory"); return nullptr; }
+    if (b->init() != 0) return nullptr;
+    return b;
+}
+
+// downsampler.lua:45-53 in global-index form: outputs sit at global input index == 0 (mod D)
+inline void decim_plan(uint64_t consumed, unsigned D, size_t n, long long* first, long long* n_out) {
+    uint64_t r = consumed % D;
+    long long f = (long long)((D - r) % D);
+    *first = f;
+    *n_out = ((long long)n > f) ? (((long long)n - f + D - 1) / D) : 0;
+}
+
+inline long long decay_samples(double c) {        // samples until |c|^k < 1e-12; < 0 if it never gets there
+    const double a = std::fabs(c);
+    if (a == 0.0) return 0;
+    if (a >= 1.0) return -1;
+    return (long long)std::ceil(std::log(1e-12) / std::log(a)) + 1;
+}
 
 struct FirFast;   // overlap-save plan (fir_fft.cu)
 struct PolyTaps;  // polyphase decimator taps (tuner.cu)
@@ -62,32 +91,31 @@ struct FirBlock : Block {
     int M = 0, D = 1;
     size_t tap_size = 4;
     std::vector<char> h_taps;
-    void* d_taps = nullptr;
-    void* d_hist[2] = {nullptr, nullptr};
+    DeviceBuffer d_taps;
+    DeviceBuffer d_hist[2];
     int cur = 0;
     int algo = 0;                     // LRB200_FIR_AUTO / DIRECT / FFT
     bool rotate = false;              // fused FrequencyTranslator in front (graph fusion; FFT path only)
     double rot_turns = 0.0;
     uint64_t rot_fix = 0;
-    FirFast* fast = nullptr;
+    FirFast* fast = nullptr;          // owned; deleted in fir_fft.cu, where the type is complete
     PolyTaps* poly = nullptr;
     bool gen_poly = false;            // poly_generic.cu covers this (kind, M, D)
     std::string label;                // owns `name` when a graph rewrite renames the block
     // output-rate pole fused behind a real polyphase decimator (graph rewrite of FIR -> IIR1 -> Downsampler)
     bool has_pole = false;
     float pole_c = 0.f;
-    void* d_pole[2] = {nullptr, nullptr};
+    DeviceBuffer d_pole[2];
     int pcur = 0;
     int set_pole(float c);
 
-    FirBlock(FirKind k, const void* taps_host, unsigned ntaps, unsigned decim, bool dev);
-    void set_rotation(double turns_per_sample) { rotate = true; rot_turns = turns_per_sample; rot_fix = turns_to_fix(turns_per_sample); }
+    // rotate: a FrequencyTranslator of turns_per_sample fused in front (graph fusion)
+    FirBlock(FirKind k, const void* taps_host, unsigned ntaps, unsigned decim, bool dev, bool rotate = false,
+             double turns_per_sample = 0.0);
     ~FirBlock() override;
     int init() override;
     size_t max_output(size_t n) const override;
     int run(const void* dx, size_t n, void* dy, size_t* n_out, cudaStream_t s) override;
-    void reset_host() override;
-    void state_buffers(std::vector<std::pair<void*, size_t>>& segs) override;
     uint64_t outputs_before(uint64_t idx) const override { return (idx + D - 1) / D; }
     long long memory_in() const override;
     void rate(unsigned* up, unsigned* down) const override { *up = 1; *down = (unsigned)D; }
@@ -95,7 +123,6 @@ struct FirBlock : Block {
     bool state_only_on_side_stream() const override { return poly != nullptr && algo != 2 && !rotate; }
     // fast paths (fir_fft.cu): fast_run returns 1 if it handled the call, 0 to fall back, <0 on error
     int fast_init();
-    void fast_free();
     int fast_run(const void* dx, size_t n, void* dy, long long first, long long n_out, cudaStream_t s);
     int set_algorithm(int a);
     int effective_algorithm() const;
@@ -110,12 +137,9 @@ struct RotatorBlock : Block {
 
 struct DiscrimBlock : Block {
     float gain = 1.f;
-    void* d_prev = nullptr;
+    DeviceBuffer d_prev;
     DiscrimBlock(float gain, bool dev);
-    ~DiscrimBlock() override;
-    int init() override;
-    void reset_host() override;
-    void state_buffers(std::vector<std::pair<void*, size_t>>& segs) override;
+    int init() override { return carry(d_prev, sizeof(float2)); }
     int run(const void* dx, size_t n, void* dy, size_t* n_out, cudaStream_t s) override;
     long long memory_in() const override { return 1; }
 };
@@ -135,16 +159,13 @@ struct IirBlock : Block {
     int nb = 1;
     float c = 0.f;
     int D = 1;                        // fused Downsampler behind the filter (graph fusion)
-    void* d_xhist[2] = {nullptr, nullptr};
-    void* d_ystate[2] = {nullptr, nullptr};
+    DeviceBuffer d_xhist[2];
+    DeviceBuffer d_ystate[2];
     int cur = 0;
     IirScanWork work;
     IirBlock(bool cplx, const float* b, unsigned nb, const float* a, unsigned na, bool dev);
-    ~IirBlock() override;
     int init() override;
     size_t max_output(size_t n) const override;
-    void reset_host() override;
-    void state_buffers(std::vector<std::pair<void*, size_t>>& segs) override;
     int run(const void* dx, size_t n, void* dy, size_t* n_out, cudaStream_t s) override;
     uint64_t outputs_before(uint64_t idx) const override { return (idx + D - 1) / D; }
     long long memory_in() const override;
@@ -157,14 +178,11 @@ struct IirGeneralBlock : Block {
     float b[10] = {0}, a[10] = {0};
     int nb = 1, na = 1;
     long long warm = -1;               // samples until the impulse response of 1/A(z) is below 1e-10 of its peak
-    void* d_xhist[2] = {nullptr, nullptr};
-    void* d_yhist[2] = {nullptr, nullptr};
+    DeviceBuffer d_xhist[2];
+    DeviceBuffer d_yhist[2];
     int cur = 0;
     IirGeneralBlock(bool cplx, const float* b, unsigned nb, const float* a, unsigned na, bool dev);
-    ~IirGeneralBlock() override;
     int init() override;
-    void reset_host() override;
-    void state_buffers(std::vector<std::pair<void*, size_t>>& segs) override;
     int run(const void* dx, size_t n, void* dy, size_t* n_out, cudaStream_t s) override;
     long long memory_in() const override { return warm < 0 ? -1 : warm + nb; }
 };
@@ -198,19 +216,16 @@ struct InterpFirBlock : Block {       // [MultiplyConstant ->] Upsampler -> FIR(
     bool has_scale;
     float scale;
     std::vector<float> h_taps;
-    float* d_taps = nullptr;
-    float* d_taps_tp = nullptr;          // [t][phase] layout for the register-tiled interpolator (D == 1, L <= 8)
+    DeviceBuffer d_taps;
+    DeviceBuffer d_taps_tp;              // [t][phase] layout for the register-tiled interpolator (D == 1, L <= 8)
     int Tt = 0;
     bool rs_ok = false;                  // the register-tiled (L, D) polyphase kernel covers this shape (resample.cu)
-    void* d_hist[2] = {nullptr, nullptr};
+    DeviceBuffer d_hist[2];
     std::string label;
     InterpFirBlock(bool cdata, const float* taps_host, int ntaps, int interp, int decim, bool has_scale, float scale, bool dev);
-    ~InterpFirBlock() override;
     int init() override;
     size_t max_output(size_t n) const override;
     uint64_t outputs_before(uint64_t idx) const override;
-    void reset_host() override { consumed = 0; cur = 0; }
-    void state_buffers(std::vector<std::pair<void*, size_t>>& segs) override;
     int run(const void* dx, size_t n, void* dy, size_t* n_out, cudaStream_t s) override;
     long long memory_in() const override { return Hn + 1; }
     void rate(unsigned* up, unsigned* down) const override { *up = (unsigned)L; *down = (unsigned)D; }
@@ -221,19 +236,18 @@ constexpr int LEVEL_MAX_TILES = 1 << 17;   // 2048-sample tiles per launch (256 
 struct LevelBlock : Block {
     bool agc = false, complex_data = false;
     double pa = 0, ga = 0, T = 0, theta = 0;  // power / gain alphas, linear target and threshold
-    void* d_state[2] = {nullptr, nullptr};    // (P, g) after the last sample, ping-ponged per launch
+    DeviceBuffer d_state[2];                  // (P, g) after the last sample, ping-ponged per launch
     int cur = 0;
-    double* d_pw = nullptr;                   // (1-ga)^k, k <= one tile
-    void* d_ticket = nullptr;                 // tile tickets, counted up across launches from ticket_base
+    DeviceBuffer d_pw;                        // (1-ga)^k, k <= one tile
+    // look-back scratch, not state: the tickets count up across launches from ticket_base and the records are tagged
+    // with epoch, both kept on the host and never reset (zeroing d_ticket alone would leave tiles waiting for ever)
+    DeviceBuffer d_ticket;                    // tile tickets
     unsigned long long ticket_base = 0;
-    void* d_rec = nullptr;                    // per-tile look-back records, 16 bytes per tile and stage
+    DeviceBuffer d_rec;                       // per-tile look-back records, 16 bytes per tile and stage
     size_t rec_bytes() const { return (size_t)16 * (agc ? 2 : 1) * LEVEL_MAX_TILES; }
     unsigned epoch = 0;
     LevelBlock(bool agc, double power_alpha, double gain_alpha, double target, double threshold, bool cplx, bool dev);
-    ~LevelBlock() override;
     int init() override;
-    void reset_host() override;
-    void state_buffers(std::vector<std::pair<void*, size_t>>& segs) override;
     int run(const void* dx, size_t n, void* dy, size_t* n_out, cudaStream_t s) override;
     long long memory_in() const override;
 };
@@ -244,6 +258,20 @@ struct LevelBlock : Block {
 struct lrb200_block_s { lrb::Block* impl; };
 
 namespace lrb {
+// a new C handle owning b; nullptr when b is (the error is set)
+inline lrb200_block_s* block_handle(std::unique_ptr<Block> b) {
+    if (!b) return nullptr;
+    lrb200_block_s* h = new (std::nothrow) lrb200_block_s{b.get()};
+    if (!h) { set_error("out of memory"); return nullptr; }
+    b.release();
+    return h;
+}
+// the lrb200_*_create tail: block B from args and the LRB200_DEVICE bit of flags, behind a new handle
+template <typename B, typename... A>
+lrb200_block_s* create_block(unsigned flags, A&&... args) {
+    return block_handle(make_block<B>(std::forward<A>(args)..., (flags & LRB200_DEVICE) != 0));
+}
+
 // tuner.cu: register-tiled polyphase decimating FIR (complex in, real taps), optional fused rotator.
 // Returns 1 if the (M, D) shape is supported and the launch was enqueued, 0 if unsupported, <0 on error.
 PolyTaps* polyphase_prepare(const float* taps, int M, int D, double turns_per_sample, bool phasor_table = false,
@@ -260,9 +288,9 @@ int launch_polyphase_rrrf(const PolyTaps* p, const float* x, const float* hist, 
 bool polyphase_pole_ok(float c);     // the pole's memory fits the kernel's warm-up
 // tuner.cu: fused FrequencyTranslator -> FIR(crcf) -> Downsampler; returns nullptr (with the error set) on failure
 // iqconv.cu: IQFileSource sample format -> ComplexFloat32 (nullptr + error for an unknown format)
-Block* make_iqconv(const char* format, bool dev);
+std::unique_ptr<Block> make_iqconv(const char* format, bool dev);
 // RealFileSource (to_file = false, comps = 1), RealFileSink/WAVFileSink (true, 1), IQFileSink (true, 2)
-Block* make_fileconv(const char* format, bool to_file, int comps, bool dev);
+std::unique_ptr<Block> make_fileconv(const char* format, bool to_file, int comps, bool dev);
 // disc_gain != 0 additionally fuses a FrequencyDiscriminator(gain) behind it (float output)
-Block* make_tuner(double turns_per_sample, const float* taps, int ntaps, int decim, float disc_gain);
+std::unique_ptr<Block> make_tuner(double turns_per_sample, const float* taps, int ntaps, int decim, float disc_gain);
 }  // namespace lrb

@@ -60,12 +60,6 @@ static int ensure_init() {
 // ---------------------------------------------------------------------------------------------
 static constexpr size_t HOST_CHUNK = (size_t)1 << 24;   // samples per staged chunk in host mode
 
-Block::~Block() {
-    cudaFree(d_in);
-    cudaFree(d_out);
-    for (void* p : m_bufs) cudaFree(p);
-}
-
 int Block::execute_multi(const void* const* x, int nin, size_t n, void* const* y, int nout, size_t* n_out) {
     cudaStream_t s = ctx().stream;
     if (nin != num_inputs || nout != num_outputs) {
@@ -78,92 +72,64 @@ int Block::execute_multi(const void* const* x, int nin, size_t n, void* const* y
         if (n_out) *n_out = produced;
         return 0;
     }
-    if (m_bufs.empty()) { m_bufs.assign((size_t)(nin + nout), nullptr); m_caps.assign((size_t)(nin + nout), 0); }
+    staging.resize((size_t)(nin + nout));
     size_t done = 0;
     std::vector<const void*> din((size_t)nin);
     std::vector<void*> dout((size_t)nout);
-    while (done < n || (n == 0 && done == 0)) {
+    while (done < n) {
         const size_t nc = n - done < HOST_CHUNK ? n - done : HOST_CHUNK;
         const size_t mo = max_output(nc);
         for (int i = 0; i < nin; ++i) {
-            if (reserve(&m_bufs[(size_t)i], &m_caps[(size_t)i], (nc ? nc : 1) * in_size) != 0) return -1;
-            if (nc) LRB_CHECK(cudaMemcpyAsync(m_bufs[(size_t)i], (const char*)x[i] + done * in_size, nc * in_size, cudaMemcpyHostToDevice, s));
-            din[(size_t)i] = m_bufs[(size_t)i];
+            DeviceBuffer& b = staging[(size_t)i];
+            if (b.reserve(nc * in_size) != 0) return -1;
+            LRB_CHECK(cudaMemcpyAsync(b.get(), (const char*)x[i] + done * in_size, nc * in_size, cudaMemcpyHostToDevice, s));
+            din[(size_t)i] = b.get();
         }
         for (int o = 0; o < nout; ++o) {
-            if (reserve(&m_bufs[(size_t)(nin + o)], &m_caps[(size_t)(nin + o)], (mo ? mo : 1) * out_size_of(o)) != 0) return -1;
-            dout[(size_t)o] = m_bufs[(size_t)(nin + o)];
+            DeviceBuffer& b = staging[(size_t)(nin + o)];
+            if (b.reserve((mo ? mo : 1) * out_size_of(o)) != 0) return -1;
+            dout[(size_t)o] = b.get();
         }
         size_t no = 0;
         if (run_multi(din.data(), nin, nc, dout.data(), nout, &no, s) != 0) return -1;
         for (int o = 0; o < nout; ++o)
             if (no) LRB_CHECK(cudaMemcpyAsync((char*)y[o] + produced * out_size_of(o), dout[(size_t)o], no * out_size_of(o), cudaMemcpyDeviceToHost, s));
+        // the staging buffers are reused by the next chunk: drain before overwriting them
         LRB_CHECK(cudaStreamSynchronize(s));
         produced += no;
         done += nc;
-        if (n == 0) break;
     }
     if (n_out) *n_out = produced;
     return 0;
 }
 
-int Block::reserve(void** p, size_t* cap, size_t bytes) {
-    if (bytes <= *cap) return 0;
-    cudaFree(*p);
-    *p = nullptr;
-    *cap = 0;
-    LRB_CHECK(cudaMalloc(p, bytes));
-    *cap = bytes;
+int Block::carry(DeviceBuffer& buf, size_t bytes) {
+    if (buf.alloc_zeroed(bytes) != 0) return -1;
+    carried.push_back({buf.get(), bytes});
     return 0;
+}
+
+int Block::carry(DeviceBuffer (&pair)[2], size_t bytes, int& cur) {
+    if (carry(pair[0], bytes) != 0 || carry(pair[1], bytes) != 0) return -1;
+    carried_index.push_back(&cur);
+    return 0;
+}
+
+void Block::rewind() {
+    consumed = 0;
+    for (int* i : carried_index) *i = 0;
 }
 
 int Block::reset() {
-    reset_host();
-    std::vector<std::pair<void*, size_t>> segs;
-    state_buffers(segs);
-    for (auto& sg : segs) LRB_CHECK(cudaMemsetAsync(sg.first, 0, sg.second, ctx().stream));
+    rewind();
+    for (auto& sg : carried) LRB_CHECK(cudaMemsetAsync(sg.first, 0, sg.second, ctx().stream));
     return 0;
-}
-
-int Block::execute(const void* x, size_t n, void* y, size_t* n_out) {
-    cudaStream_t s = ctx().stream;
-    size_t produced = 0;
-    if (dev_ptrs) {
-        if (run(x, n, y, &produced, s) != 0) return -1;
-        if (n_out) *n_out = produced;
-        return 0;
-    }
-    size_t done = 0;
-    while (done < n) {
-        size_t nc = n - done < HOST_CHUNK ? n - done : HOST_CHUNK;
-        size_t mo = max_output(nc);
-        if (reserve(&d_in, &d_in_cap, nc * in_size) != 0) return -1;
-        if (reserve(&d_out, &d_out_cap, (mo ? mo : 1) * out_size) != 0) return -1;
-        LRB_CHECK(cudaMemcpyAsync(d_in, (const char*)x + done * in_size, nc * in_size, cudaMemcpyHostToDevice, s));
-        size_t no = 0;
-        if (run(d_in, nc, d_out, &no, s) != 0) return -1;
-        if (no) LRB_CHECK(cudaMemcpyAsync((char*)y + produced * out_size, d_out, no * out_size, cudaMemcpyDeviceToHost, s));
-        // the staging buffers are reused by the next chunk: drain before overwriting d_in
-        LRB_CHECK(cudaStreamSynchronize(s));
-        produced += no;
-        done += nc;
-    }
-    if (n_out) *n_out = produced;
-    return 0;
-}
-
-static inline void decim_plan(uint64_t consumed, unsigned D, size_t n, long long* first, long long* n_out) {
-    // downsampler.lua:45-53 in global-index form: outputs sit at global input index == 0 (mod D)
-    uint64_t r = consumed % D;
-    long long f = (long long)((D - r) % D);
-    *first = f;
-    *n_out = ((long long)n > f) ? (((long long)n - f + D - 1) / D) : 0;
 }
 
 // ---------------------------------------------------------------------------------------------
 // FIR (+ Hilbert)
 // ---------------------------------------------------------------------------------------------
-FirBlock::FirBlock(FirKind k, const void* taps_host, unsigned ntaps, unsigned decim, bool dev) {
+FirBlock::FirBlock(FirKind k, const void* taps_host, unsigned ntaps, unsigned decim, bool dev, bool rot, double turns_per_sample) {
     kind = k;
     M = (int)ntaps;
     D = (int)decim;
@@ -173,47 +139,30 @@ FirBlock::FirBlock(FirKind k, const void* taps_host, unsigned ntaps, unsigned de
     out_size = (cin || k == FIR_HILBERT) ? 8 : 4;
     tap_size = (k == FIR_CCCF) ? 8 : 4;
     name = k == FIR_CRCF ? "fir_crcf" : k == FIR_CCCF ? "fir_cccf" : k == FIR_RRRF ? "fir_rrrf" : "hilbert";
+    if (rot) {
+        // (the fused translator forces the overlap-save path: algo is moot)
+        rotate = true;
+        rot_turns = turns_per_sample;
+        rot_fix = turns_to_fix(turns_per_sample);
+        name = k == FIR_CCCF ? "rot+fir_cccf" : "rot+fir_crcf";
+    }
     h_taps.assign((const char*)taps_host, (const char*)taps_host + (size_t)M * tap_size);
 }
 
 int FirBlock::init() {
-    LRB_CHECK(cudaMalloc(&d_taps, (size_t)M * tap_size));
-    LRB_CHECK(cudaMemcpy(d_taps, h_taps.data(), (size_t)M * tap_size, cudaMemcpyHostToDevice));
-    size_t hb = (size_t)(M > 1 ? M - 1 : 1) * in_size;
-    for (int i = 0; i < 2; ++i) {
-        LRB_CHECK(cudaMalloc(&d_hist[i], hb));
-        LRB_CHECK(cudaMemset(d_hist[i], 0, hb));
-    }
+    if (d_taps.upload(h_taps.data(), (size_t)M * tap_size) != 0) return -1;
+    if (carry(d_hist, (size_t)(M > 1 ? M - 1 : 1) * in_size, cur) != 0) return -1;
     return fast_init();
 }
 
 int FirBlock::set_pole(float c) {
-    for (int i = 0; i < 2; ++i) {
-        LRB_CHECK(cudaMalloc(&d_pole[i], sizeof(float)));
-        LRB_CHECK(cudaMemset(d_pole[i], 0, sizeof(float)));
-    }
+    if (carry(d_pole, sizeof(float), pcur) != 0) return -1;
     has_pole = true;
     pole_c = c;
     return 0;
 }
 
-FirBlock::~FirBlock() {
-    cudaFree(d_pole[0]);
-    cudaFree(d_pole[1]);
-    cudaFree(d_taps);
-    cudaFree(d_hist[0]);
-    cudaFree(d_hist[1]);
-    fast_free();
-}
-
 size_t FirBlock::max_output(size_t n) const { return D == 1 ? n : n / D + 1; }
-
-static long long decay_samples(double c) {        // samples until |c|^k < 1e-12; < 0 if it never gets there
-    const double a = std::fabs(c);
-    if (a == 0.0) return 0;
-    if (a >= 1.0) return -1;
-    return (long long)std::ceil(std::log(1e-12) / std::log(a)) + 1;
-}
 
 long long FirBlock::memory_in() const {
     long long m = M - 1;
@@ -229,14 +178,6 @@ long long IirBlock::memory_in() const {
     return w < 0 ? -1 : w + nb;
 }
 
-void FirBlock::reset_host() { consumed = 0; cur = 0; pcur = 0; }
-void FirBlock::state_buffers(std::vector<std::pair<void*, size_t>>& segs) {
-    const size_t hb = (size_t)(M > 1 ? M - 1 : 1) * in_size;
-    segs.push_back({d_hist[0], hb});
-    segs.push_back({d_hist[1], hb});
-    if (has_pole) { segs.push_back({d_pole[0], sizeof(float)}); segs.push_back({d_pole[1], sizeof(float)}); }
-}
-
 int FirBlock::run(const void* dx, size_t n, void* dy, size_t* n_out, cudaStream_t s) {
     long long first, no;
     decim_plan(consumed, (unsigned)D, n, &first, &no);
@@ -247,10 +188,10 @@ int FirBlock::run(const void* dx, size_t n, void* dy, size_t* n_out, cudaStream_
     cudaStream_t side = s;
     if (M > 1) {
         if (n >= SIDE_STREAM_MIN) side = side_fork(s);
-        if (launch_hist_update(dx, (long long)n, d_hist[cur], d_hist[cur ^ 1], M - 1, (int)in_size, side) != 0) return -1;
+        if (launch_hist_update(dx, (long long)n, d_hist[cur].get(), d_hist[cur ^ 1].get(), M - 1, (int)in_size, side) != 0) return -1;
     }
     int rc = fast_run(dx, n, dy, first, no, s);
-    if (rc == 0) rc = launch_fir_generic(kind, dx, d_hist[cur], d_taps, M, D, first, no, dy, s) == 0 ? 1 : -1;
+    if (rc == 0) rc = launch_fir_generic(kind, dx, d_hist[cur].get(), d_taps.get(), M, D, first, no, dy, s) == 0 ? 1 : -1;
     side_join(s, side);
     if (rc < 0) return -1;
     if (M > 1) cur ^= 1;
@@ -287,19 +228,11 @@ DiscrimBlock::DiscrimBlock(float gain_, bool dev) {
     dev_ptrs = dev;
     gain = gain_;
 }
-int DiscrimBlock::init() {
-    LRB_CHECK(cudaMalloc(&d_prev, sizeof(float2)));
-    LRB_CHECK(cudaMemset(d_prev, 0, sizeof(float2)));
-    return 0;
-}
-DiscrimBlock::~DiscrimBlock() { cudaFree(d_prev); }
-void DiscrimBlock::reset_host() { consumed = 0; }
-void DiscrimBlock::state_buffers(std::vector<std::pair<void*, size_t>>& segs) { segs.push_back({d_prev, sizeof(float2)}); }
 int DiscrimBlock::run(const void* dx, size_t n, void* dy, size_t* n_out, cudaStream_t s) {
     *n_out = n;
     if (n == 0) return 0;
-    if (launch_discrim((const float2*)dx, (const float2*)d_prev, (float*)dy, (long long)n, 1.0f / gain, s) != 0) return -1;
-    if (launch_copy_last(dx, (long long)n, d_prev, 8, s) != 0) return -1;
+    if (launch_discrim((const float2*)dx, d_prev.as<const float2>(), (float*)dy, (long long)n, 1.0f / gain, s) != 0) return -1;
+    if (launch_copy_last(dx, (long long)n, d_prev.get(), 8, s) != 0) return -1;
     consumed += n;
     return 0;
 }
@@ -337,25 +270,10 @@ IirBlock::IirBlock(bool cplx, const float* b_, unsigned nb_, const float* a_, un
     c = (na_ >= 2) ? (float)(-(double)a_[1] / a0) : 0.0f;
 }
 int IirBlock::init() {
-    size_t hb = (size_t)(nb > 1 ? nb - 1 : 1) * in_size;
-    for (int i = 0; i < 2; ++i) {
-        LRB_CHECK(cudaMalloc(&d_xhist[i], hb));
-        LRB_CHECK(cudaMemset(d_xhist[i], 0, hb));
-        LRB_CHECK(cudaMalloc(&d_ystate[i], in_size));
-        LRB_CHECK(cudaMemset(d_ystate[i], 0, in_size));
-    }
+    if (carry(d_xhist, (size_t)(nb > 1 ? nb - 1 : 1) * in_size, cur) != 0 || carry(d_ystate, in_size, cur) != 0) return -1;
     return iir_work_alloc(&work, (int)in_size);
 }
-IirBlock::~IirBlock() {
-    for (int i = 0; i < 2; ++i) { cudaFree(d_xhist[i]); cudaFree(d_ystate[i]); }
-    iir_work_free(&work);
-}
 size_t IirBlock::max_output(size_t n) const { return D == 1 ? n : n / D + 1; }
-void IirBlock::reset_host() { consumed = 0; cur = 0; }
-void IirBlock::state_buffers(std::vector<std::pair<void*, size_t>>& segs) {
-    const size_t hb = (size_t)(nb > 1 ? nb - 1 : 1) * in_size;
-    for (int i = 0; i < 2; ++i) { segs.push_back({d_xhist[i], hb}); segs.push_back({d_ystate[i], in_size}); }
-}
 int IirBlock::run(const void* dx, size_t n, void* dy, size_t* n_out, cudaStream_t s) {
     long long first_total, no_total;
     decim_plan(consumed, (unsigned)D, n, &first_total, &no_total);
@@ -367,7 +285,7 @@ int IirBlock::run(const void* dx, size_t n, void* dy, size_t* n_out, cudaStream_
         long long first, no;
         decim_plan(consumed, (unsigned)D, (size_t)nc, &first, &no);
         if (launch_iir1(complex_data, (const char*)dx + done * in_size, nc, (char*)dy + produced * out_size, b, nb, c,
-                        d_xhist[cur], d_xhist[cur ^ 1], d_ystate[cur], d_ystate[cur ^ 1], first, D, &work, s) != 0)
+                        d_xhist[cur].get(), d_xhist[cur ^ 1].get(), d_ystate[cur].get(), d_ystate[cur ^ 1].get(), first, D, &work, s) != 0)
             return -1;
         cur ^= 1;
         consumed += (uint64_t)nc;
@@ -406,28 +324,15 @@ IirGeneralBlock::IirGeneralBlock(bool cplx, const float* b_, unsigned nb_, const
     warm = (last + na + nb >= limit - 1) ? -1 : last + na + nb;
 }
 int IirGeneralBlock::init() {
-    for (int i = 0; i < 2; ++i) {
-        LRB_CHECK(cudaMalloc(&d_xhist[i], 10 * in_size));
-        LRB_CHECK(cudaMemset(d_xhist[i], 0, 10 * in_size));
-        LRB_CHECK(cudaMalloc(&d_yhist[i], 10 * in_size));
-        LRB_CHECK(cudaMemset(d_yhist[i], 0, 10 * in_size));
-    }
-    return 0;
-}
-IirGeneralBlock::~IirGeneralBlock() {
-    for (int i = 0; i < 2; ++i) { cudaFree(d_xhist[i]); cudaFree(d_yhist[i]); }
-}
-void IirGeneralBlock::reset_host() { consumed = 0; cur = 0; }
-void IirGeneralBlock::state_buffers(std::vector<std::pair<void*, size_t>>& segs) {
-    for (int i = 0; i < 2; ++i) { segs.push_back({d_xhist[i], 10 * in_size}); segs.push_back({d_yhist[i], 10 * in_size}); }
+    return carry(d_xhist, 10 * in_size, cur) != 0 || carry(d_yhist, 10 * in_size, cur) != 0 ? -1 : 0;
 }
 int IirGeneralBlock::run(const void* dx, size_t n, void* dy, size_t* n_out, cudaStream_t s) {
     *n_out = n;
     if (n == 0) return 0;
-    if (launch_iir_general(complex_data, dx, (long long)n, dy, b, nb, a, na, d_xhist[cur], d_yhist[cur], warm, s) != 0) return -1;
+    if (launch_iir_general(complex_data, dx, (long long)n, dy, b, nb, a, na, d_xhist[cur].get(), d_yhist[cur].get(), warm, s) != 0) return -1;
     // carried state: last nb-1 inputs of [xhist | x], last na-1 outputs of [yhist | y] (oldest first)
-    if (nb > 1 && launch_hist_update(dx, (long long)n, d_xhist[cur], d_xhist[cur ^ 1], nb - 1, (int)in_size, s) != 0) return -1;
-    if (na > 1 && launch_hist_update(dy, (long long)n, d_yhist[cur], d_yhist[cur ^ 1], na - 1, (int)in_size, s) != 0) return -1;
+    if (nb > 1 && launch_hist_update(dx, (long long)n, d_xhist[cur].get(), d_xhist[cur ^ 1].get(), nb - 1, (int)in_size, s) != 0) return -1;
+    if (na > 1 && launch_hist_update(dy, (long long)n, d_yhist[cur].get(), d_yhist[cur ^ 1].get(), na - 1, (int)in_size, s) != 0) return -1;
     cur ^= 1;
     consumed += n;
     return 0;
@@ -456,16 +361,6 @@ int C2fBlock::run(const void* dx, size_t n, void* dy, size_t* n_out, cudaStream_
 // extern "C" surface
 // =============================================================================================
 using namespace lrb;
-
-
-template <typename B>
-static lrb200_block_t* wrap(B* b) {
-    if (!b) { set_error("out of memory"); return nullptr; }
-    if (b->init() != 0) { delete b; return nullptr; }
-    lrb200_block_t* h = new (std::nothrow) lrb200_block_s{b};
-    if (!h) { delete b; set_error("out of memory"); }
-    return h;
-}
 
 extern "C" {
 
@@ -638,7 +533,7 @@ static lrb200_block_t* fir_create(FirKind k, const void* taps, unsigned ntaps, u
     if (!taps || ntaps == 0) { set_error("fir: taps must be non-empty"); return nullptr; }
     if (decim == 0) { set_error("fir: decimation must be >= 1"); return nullptr; }
     if (k == FIR_HILBERT && (ntaps % 2) == 0) { set_error("hilbert: number of taps must be odd"); return nullptr; }
-    return wrap(new (std::nothrow) FirBlock(k, taps, ntaps, decim, (flags & LRB200_DEVICE) != 0));
+    return create_block<FirBlock>(flags, k, taps, ntaps, decim);
 }
 lrb200_fir_t* lrb200_fir_create_crcf(const float32_t* taps, unsigned ntaps, unsigned decim, unsigned flags) { return fir_create(FIR_CRCF, taps, ntaps, decim, flags); }
 lrb200_fir_t* lrb200_fir_create_cccf(const complex_float32_t* taps, unsigned ntaps, unsigned decim, unsigned flags) { return fir_create(FIR_CCCF, taps, ntaps, decim, flags); }
@@ -662,20 +557,20 @@ lrb200_hilbert_t* lrb200_hilbert_create(const float32_t* taps, unsigned ntaps, u
 lrb200_rotator_t* lrb200_rotator_create(double turns_per_sample, unsigned flags) {
     if (ensure_init() != 0) return nullptr;
     if (!std::isfinite(turns_per_sample)) { set_error("rotator: turns_per_sample is not finite"); return nullptr; }
-    return wrap(new (std::nothrow) RotatorBlock(turns_per_sample, (flags & LRB200_DEVICE) != 0));
+    return create_block<RotatorBlock>(flags, turns_per_sample);
 }
 
 lrb200_discrim_t* lrb200_discrim_create(float gain, unsigned flags) {
     if (ensure_init() != 0) return nullptr;
     if (!(gain != 0.0f) || !std::isfinite(gain)) { set_error("discrim: gain must be finite and non-zero"); return nullptr; }
-    return wrap(new (std::nothrow) DiscrimBlock(gain, (flags & LRB200_DEVICE) != 0));
+    return create_block<DiscrimBlock>(flags, gain);
 }
 
 lrb200_downsample_t* lrb200_downsample_create(unsigned factor, unsigned elem_size, unsigned flags) {
     if (ensure_init() != 0) return nullptr;
     if (factor == 0) { set_error("downsample: factor must be >= 1"); return nullptr; }
     if (elem_size != 4 && elem_size != 8) { set_error("downsample: elem_size must be 4 or 8"); return nullptr; }
-    return wrap(new (std::nothrow) DownsampleBlock(factor, elem_size, (flags & LRB200_DEVICE) != 0));
+    return create_block<DownsampleBlock>(flags, factor, elem_size);
 }
 
 static lrb200_block_t* iir_create(bool cplx, const float32_t* b, unsigned nb, const float32_t* a, unsigned na, unsigned flags) {
@@ -684,54 +579,49 @@ static lrb200_block_t* iir_create(bool cplx, const float32_t* b, unsigned nb, co
     if (nb > 10 || na > 10) { set_error("iir: at most 10 feed-forward and 10 feedback taps"); return nullptr; }
     if (a[0].value == 0.0f) { set_error("iir: a[0] must be non-zero"); return nullptr; }
     if (na > 2 || nb > 9)
-        return wrap(new (std::nothrow) IirGeneralBlock(cplx, (const float*)b, nb, (const float*)a, na, (flags & LRB200_DEVICE) != 0));
-    return wrap(new (std::nothrow) IirBlock(cplx, (const float*)b, nb, (const float*)a, na, (flags & LRB200_DEVICE) != 0));
+        return create_block<IirGeneralBlock>(flags, cplx, (const float*)b, nb, (const float*)a, na);
+    return create_block<IirBlock>(flags, cplx, (const float*)b, nb, (const float*)a, na);
 }
 lrb200_iir_t* lrb200_iir_create_rrrf(const float32_t* b, unsigned nb, const float32_t* a, unsigned na, unsigned flags) { return iir_create(false, b, nb, a, na, flags); }
 lrb200_iir_t* lrb200_iir_create_crcf(const float32_t* b, unsigned nb, const float32_t* a, unsigned na, unsigned flags) { return iir_create(true, b, nb, a, na, flags); }
 
 lrb200_block_t* lrb200_cmag_create(unsigned flags) {
     if (ensure_init() != 0) return nullptr;
-    return wrap(new (std::nothrow) C2fBlock(0, (flags & LRB200_DEVICE) != 0));
+    return create_block<C2fBlock>(flags, 0);
 }
 lrb200_block_t* lrb200_c2r_create(unsigned flags) {
     if (ensure_init() != 0) return nullptr;
-    return wrap(new (std::nothrow) C2fBlock(1, (flags & LRB200_DEVICE) != 0));
+    return create_block<C2fBlock>(flags, 1);
 }
 
 lrb200_block_t* lrb200_mulconst_create(float re, float im, unsigned complex_data, unsigned complex_constant, unsigned flags) {
     if (ensure_init() != 0) return nullptr;
     if (complex_constant && !complex_data) { set_error("mulconst: a complex constant needs complex data"); return nullptr; }
-    return wrap(new (std::nothrow) ScaleBlock(re, im, complex_data != 0, complex_constant != 0, (flags & LRB200_DEVICE) != 0));
+    return create_block<ScaleBlock>(flags, re, im, complex_data != 0, complex_constant != 0);
 }
 lrb200_block_t* lrb200_upsample_create(unsigned factor, unsigned elem_size, unsigned flags) {
     if (ensure_init() != 0) return nullptr;
     if (factor == 0) { set_error("upsample: factor must be >= 1"); return nullptr; }
     if (elem_size != 4 && elem_size != 8) { set_error("upsample: elem_size must be 4 or 8"); return nullptr; }
-    return wrap(new (std::nothrow) UpsampleBlock(factor, elem_size, (flags & LRB200_DEVICE) != 0));
+    return create_block<UpsampleBlock>(flags, factor, elem_size);
 }
 
 lrb200_block_t* lrb200_iqconv_create(const char* format, unsigned flags) {
     if (ensure_init() != 0) return nullptr;
-    Block* b = make_iqconv(format, (flags & LRB200_DEVICE) != 0);
-    if (!b) return nullptr;
-    return wrap(b);
+    return block_handle(make_iqconv(format, (flags & LRB200_DEVICE) != 0));
 }
 
 lrb200_block_t* lrb200_realconv_create(const char* format, unsigned flags) {
     if (ensure_init() != 0) return nullptr;
-    Block* b = make_fileconv(format, false, 1, (flags & LRB200_DEVICE) != 0);
-    return b ? wrap(b) : nullptr;
+    return block_handle(make_fileconv(format, false, 1, (flags & LRB200_DEVICE) != 0));
 }
 lrb200_block_t* lrb200_iqsink_create(const char* format, unsigned flags) {
     if (ensure_init() != 0) return nullptr;
-    Block* b = make_fileconv(format, true, 2, (flags & LRB200_DEVICE) != 0);
-    return b ? wrap(b) : nullptr;
+    return block_handle(make_fileconv(format, true, 2, (flags & LRB200_DEVICE) != 0));
 }
 lrb200_block_t* lrb200_realsink_create(const char* format, unsigned flags) {
     if (ensure_init() != 0) return nullptr;
-    Block* b = make_fileconv(format, true, 1, (flags & LRB200_DEVICE) != 0);
-    return b ? wrap(b) : nullptr;
+    return block_handle(make_fileconv(format, true, 1, (flags & LRB200_DEVICE) != 0));
 }
 
 // ---- level control -----------------------------------------------------------------------------
@@ -749,8 +639,7 @@ lrb200_block_t* lrb200_agc_create(double target_dbfs, double threshold_dbfs, dou
     const double gain_alpha = 1 / (1 + gain_tau * rate);
     const double target = std::pow(10.0, target_dbfs / 10);
     const double threshold = std::pow(10.0, threshold_dbfs / 10);
-    return wrap(new (std::nothrow) LevelBlock(true, power_alpha, gain_alpha, target, threshold, complex_data != 0,
-                                              (flags & LRB200_DEVICE) != 0));
+    return create_block<LevelBlock>(flags, true, power_alpha, gain_alpha, target, threshold, complex_data != 0);
 }
 
 lrb200_block_t* lrb200_powersquelch_create(double threshold_dbfs, double tau, double rate, unsigned complex_data, unsigned flags) {
@@ -761,7 +650,7 @@ lrb200_block_t* lrb200_powersquelch_create(double threshold_dbfs, double tau, do
     // powersquelch.lua:34-38
     const double alpha = 1 / (1 + tau * rate);
     const double threshold = std::pow(10.0, threshold_dbfs / 10);
-    return wrap(new (std::nothrow) LevelBlock(false, alpha, 0.0, 0.0, threshold, complex_data != 0, (flags & LRB200_DEVICE) != 0));
+    return create_block<LevelBlock>(flags, false, alpha, 0.0, 0.0, threshold, complex_data != 0);
 }
 
 // ---- synthetic sources -------------------------------------------------------------------------

@@ -38,6 +38,47 @@ bool cuda_ok(cudaError_t e, const char* what);
         if (!::lrb::cuda_ok((call), #call)) return -1;    \
     } while (0)
 
+// One cudaMalloc region, freed with the object.  The int-returning members follow LRB_CHECK: 0, or -1 with the error set.
+class DeviceBuffer {
+public:
+    DeviceBuffer() = default;
+    DeviceBuffer(const DeviceBuffer&) = delete;
+    DeviceBuffer& operator=(const DeviceBuffer&) = delete;
+    DeviceBuffer(DeviceBuffer&& o) noexcept : p_(o.p_), cap_(o.cap_) { o.p_ = nullptr; o.cap_ = 0; }
+    DeviceBuffer& operator=(DeviceBuffer&& o) noexcept {
+        if (this != &o) { cudaFree(p_); p_ = o.p_; cap_ = o.cap_; o.p_ = nullptr; o.cap_ = 0; }
+        return *this;
+    }
+    ~DeviceBuffer() { cudaFree(p_); }
+    void* get() const { return p_; }
+    template <typename T> T* as() const { return static_cast<T*>(p_); }
+    size_t capacity() const { return cap_; }
+    // grow-only (like Vector:resize): a larger request drops the contents and allocates anew
+    int reserve(size_t bytes) {
+        if (bytes <= cap_) return 0;
+        cudaFree(p_);
+        p_ = nullptr;
+        cap_ = 0;
+        LRB_CHECK(cudaMalloc(&p_, bytes));
+        cap_ = bytes;
+        return 0;
+    }
+    int alloc_zeroed(size_t bytes) {
+        if (reserve(bytes) != 0) return -1;
+        LRB_CHECK(cudaMemset(p_, 0, bytes));
+        return 0;
+    }
+    int upload(const void* host, size_t bytes) {
+        if (reserve(bytes) != 0) return -1;
+        LRB_CHECK(cudaMemcpy(p_, host, bytes, cudaMemcpyHostToDevice));
+        return 0;
+    }
+
+private:
+    void* p_ = nullptr;
+    size_t cap_ = 0;
+};
+
 // cycles-per-sample (any sign / magnitude) -> fraction of a turn in 2^-64 units.  Done in 80-bit long double
 // so that removing the integer part does not round the 53-bit fraction (a 2^-54 error per sample is
 // 3e-6 rad after 2^33 samples).
@@ -90,15 +131,14 @@ int launch_zero_segments(void* const* ptrs, const size_t* bytes, int count, cuda
 // ping-ponged by the caller: *_in is read, *_out written.  Fused decimation: only outputs whose
 // index (first + j*D) are written when D > 1.
 struct IirScanWork {           // device-side scratch for the decoupled look-back
-    int* ticket = nullptr;     // 1 int
-    int* flags = nullptr;      // max_tiles ints
-    void* agg = nullptr;       // max_tiles elements
-    void* pfx = nullptr;       // max_tiles elements
+    DeviceBuffer ticket;       // 1 int
+    DeviceBuffer flags;        // max_tiles ints
+    DeviceBuffer agg;          // max_tiles elements
+    DeviceBuffer pfx;          // max_tiles elements
     int max_tiles = 0;
     unsigned epoch = 0;
 };
 int iir_work_alloc(IirScanWork* w, int elem_size);
-void iir_work_free(IirScanWork* w);
 long long iir_max_per_launch(const IirScanWork& w);
 int launch_iir1(bool complex_data, const void* x, long long n, void* y, const float* b_host, int nb, float c,
                 const void* xhist_in, void* xhist_out, const void* ystate_in, void* ystate_out,

@@ -531,9 +531,9 @@ int launch_fdl(const FdlArgs& a, cudaStream_t s) {
 struct FirFast {
     int nparts = 1;            // > 1: uniformly partitioned overlap-save for filters longer than one block allows
     int part_taps = 0;
-    float2* d_H = nullptr;     // nparts tap spectra, FF_N each
-    float2* d_tw = nullptr;
-    float2* d_E = nullptr;
+    DeviceBuffer d_H;          // nparts tap spectra, FF_N each
+    DeviceBuffer d_tw;
+    DeviceBuffer d_E;
     int in_mode = 0;
 };
 
@@ -582,10 +582,8 @@ int FirBlock::fast_init() {
             const int e = (a * c) % FF_N;
             tw[a * 32 + c] = make_float2((float)std::cos(two_pi * e / FF_N), (float)(-std::sin(two_pi * e / FF_N)));
         }
-    LRB_CHECK(cudaMalloc(&fast->d_H, sizeof(float2) * H.size()));
-    LRB_CHECK(cudaMalloc(&fast->d_tw, sizeof(float2) * FF_N));
-    LRB_CHECK(cudaMemcpy(fast->d_H, H.data(), sizeof(float2) * H.size(), cudaMemcpyHostToDevice));
-    LRB_CHECK(cudaMemcpy(fast->d_tw, tw.data(), sizeof(float2) * FF_N, cudaMemcpyHostToDevice));
+    if (fast->d_H.upload(H.data(), sizeof(float2) * H.size()) != 0 || fast->d_tw.upload(tw.data(), sizeof(float2) * FF_N) != 0)
+        return -1;
     if (rotate) {
         // E[n] = exp(j 2 pi turns n) from the same 2^-64 fixed-point turns the kernel uses for the block phasor
         const long double tq = ldexpl((long double)rot_fix, -64);
@@ -594,22 +592,14 @@ int FirBlock::fast_init() {
             a -= floorl(a);
             E[i] = make_float2((float)std::cos(two_pi * (double)a), (float)std::sin(two_pi * (double)a));
         }
-        LRB_CHECK(cudaMalloc(&fast->d_E, sizeof(float2) * FF_N));
-        LRB_CHECK(cudaMemcpy(fast->d_E, E.data(), sizeof(float2) * FF_N, cudaMemcpyHostToDevice));
+        if (fast->d_E.upload(E.data(), sizeof(float2) * FF_N) != 0) return -1;
     }
     return 0;
 }
 
-void FirBlock::fast_free() {
+FirBlock::~FirBlock() {
     polyphase_release(poly);
-    poly = nullptr;
-    if (fast) {
-        cudaFree(fast->d_H);
-        cudaFree(fast->d_tw);
-        cudaFree(fast->d_E);
-        delete fast;
-        fast = nullptr;
-    }
+    delete fast;
 }
 
 // The algorithm that would run for a long input (what lrb200_fir_get_algorithm reports).
@@ -638,15 +628,15 @@ int FirBlock::set_algorithm(int a) {
 
 int FirBlock::fast_run(const void* dx, size_t n, void* dy, long long first, long long n_out, cudaStream_t s) {
     if (poly && algo != LRB200_FIR_FFT && kind == FIR_RRRF)
-        return launch_polyphase_rrrf(poly, (const float*)dx, (const float*)d_hist[cur], (long long)n, (float*)dy, first, n_out, s,
-                                     pole_c, has_pole ? (const float*)d_pole[pcur] : nullptr, has_pole ? (float*)d_pole[pcur ^ 1] : nullptr);
+        return launch_polyphase_rrrf(poly, (const float*)dx, d_hist[cur].as<const float>(), (long long)n, (float*)dy, first, n_out, s,
+                                     pole_c, d_pole[pcur].as<const float>(), d_pole[pcur ^ 1].as<float>());
     if (has_pole) { set_error("fir: the fused output-rate pole needs the real polyphase kernel"); return -1; }
     if (poly && algo != LRB200_FIR_FFT)
-        return launch_polyphase_crcf(poly, (const float2*)dx, (const float2*)d_hist[cur], (long long)n, (float2*)dy,
+        return launch_polyphase_crcf(poly, (const float2*)dx, d_hist[cur].as<const float2>(), (long long)n, (float2*)dy,
                                      first, n_out, false, 0, consumed, s);
     const int eff = effective_algorithm();
     if (gen_poly && eff == LRB200_FIR_DIRECT) {
-        const int rc = launch_poly_generic(kind, dx, d_hist[cur], h_taps.data(), M, D, first, (long long)n, n_out, dy, s);
+        const int rc = launch_poly_generic(kind, dx, d_hist[cur].get(), h_taps.data(), M, D, first, (long long)n, n_out, dy, s);
         if (rc != 0) return rc;
     }
     if (!fast || eff != LRB200_FIR_FFT) {
@@ -665,8 +655,8 @@ int FirBlock::fast_run(const void* dx, size_t n, void* dy, long long first, long
         const long long nb = ((long long)n + FD_HOP - 1) / FD_HOP;
         for (int p0 = 0; p0 < fast->nparts; p0 += FD_MAXPC) {
             FdlArgs a;
-            a.x = (const float2*)dx; a.hist = (const float2*)d_hist[cur]; a.y = (float2*)dy;
-            a.H = fast->d_H + (size_t)p0 * FF_N; a.tw = fast->d_tw; a.n = (long long)n;
+            a.x = (const float2*)dx; a.hist = d_hist[cur].as<const float2>(); a.y = (float2*)dy;
+            a.H = fast->d_H.as<float2>() + (size_t)p0 * FF_N; a.tw = fast->d_tw.as<float2>(); a.n = (long long)n;
             a.pc = std::min(FD_MAXPC, fast->nparts - p0);
             a.nblocks = nb;
             a.b_lo = std::min<long long>(nb, a.pc + p0);          // first block whose ring pre-fill reads x[>= 0]
@@ -686,7 +676,7 @@ int FirBlock::fast_run(const void* dx, size_t n, void* dy, long long first, long
         if (b_hi < b_lo) b_hi = b_lo;
         if (b_lo > nblocks) { b_lo = nblocks; b_hi = nblocks; }
         FftArgs a;
-        a.x = dx; a.hist = d_hist[cur]; a.y = dy; a.H = fast->d_H; a.tw = fast->d_tw; a.E = fast->d_E;
+        a.x = dx; a.hist = d_hist[cur].get(); a.y = dy; a.H = fast->d_H.as<float2>(); a.tw = fast->d_tw.as<float2>(); a.E = fast->d_E.as<float2>();
         a.n = (long long)n; a.b_lo = b_lo; a.b_hi = b_hi; a.nwork = 0; a.first = first;
         a.turns_fix = rot_fix; a.g0 = consumed; a.M = Mp; a.D = D;
         // edge work list: blocks [0, b_lo) and [b_hi, nblocks); the kernel maps e -> (e < b_lo ? e : b_hi + e - b_lo)

@@ -16,6 +16,7 @@
 #include <cmath>
 #include <cstdlib>
 #include <cstring>
+#include <memory>
 #include <new>
 #include <string>
 #include <vector>
@@ -23,15 +24,13 @@
 namespace lrb {
 
 struct Graph {
-    std::vector<Block*> blocks;      // as appended (owned)
-    std::vector<Block*> fused;       // blocks created by fusion (owned)
+    std::vector<std::unique_ptr<Block>> blocks;   // as appended
+    std::vector<std::unique_ptr<Block>> fused;    // blocks created by fusion
     std::vector<Block*> stages;      // execution order after commit (not owned)
     bool committed = false;
-    void* ring[2] = {nullptr, nullptr};
-    size_t ring_cap[2] = {0, 0};
+    DeviceBuffer ring[2];
     // host-mode double buffering
-    void* d_in[2] = {nullptr, nullptr};  size_t d_in_cap[2] = {0, 0};
-    void* d_out[2] = {nullptr, nullptr}; size_t d_out_cap[2] = {0, 0};
+    DeviceBuffer d_in[2], d_out[2];
     cudaStream_t s_h2d = nullptr, s_d2h = nullptr;
     cudaEvent_t ev_h2d[2] = {nullptr, nullptr}, ev_comp[2] = {nullptr, nullptr}, ev_d2h[2] = {nullptr, nullptr};
     size_t host_chunk = (size_t)1 << 23;   // input samples per pipelined chunk
@@ -39,18 +38,18 @@ struct Graph {
     // super-chunk mode (SURVEY.md 8e "streaming mode"): small host vectors are packed into pinned slots of `sc` samples;
     // a full slot is processed asynchronously while the next one fills, and its outputs are handed back when that next
     // slot is submitted (or at flush) -- the per-vector cost is one host memcpy instead of copies + launches + a sync
+    struct HostFree { void operator()(char* p) const { cudaFreeHost(p); } };
+    using PinnedSlot = std::unique_ptr<char, HostFree>;
     size_t sc = 0;
-    char* sc_hin[2] = {nullptr, nullptr};
-    char* sc_hout[2] = {nullptr, nullptr};
-    void* sc_din[2] = {nullptr, nullptr};
-    void* sc_dout[2] = {nullptr, nullptr};
+    PinnedSlot sc_hin[2], sc_hout[2];
+    DeviceBuffer sc_din[2], sc_dout[2];
     cudaEvent_t sc_done[2] = {nullptr, nullptr};
     bool sc_pending[2] = {false, false};
     size_t sc_nout[2] = {0, 0};
     size_t sc_fill = 0, sc_outcap = 0;
     int sc_cur = 0;
     // time-chunk sharding (run_shard): scratch for the outputs that belong to the halo
-    void* head_out = nullptr; size_t head_out_cap = 0;
+    DeviceBuffer head_out;
     // optional per-stage timing
     bool timing = false;
     std::vector<std::vector<cudaEvent_t>> tev;   // per stage: [start0, stop0, start1, stop1, ...]
@@ -65,10 +64,7 @@ struct Graph {
 
     ~Graph() {
         for (auto& v : tev) for (cudaEvent_t e : v) cudaEventDestroy(e);
-        for (Block* b : blocks) delete b;
-        for (Block* b : fused) delete b;
         for (int i = 0; i < 2; ++i) {
-            cudaFree(ring[i]); cudaFree(d_in[i]); cudaFree(d_out[i]);
             if (ev_h2d[i]) cudaEventDestroy(ev_h2d[i]);
             if (ev_comp[i]) cudaEventDestroy(ev_comp[i]);
             if (ev_d2h[i]) cudaEventDestroy(ev_d2h[i]);
@@ -76,16 +72,14 @@ struct Graph {
         if (s_h2d) cudaStreamDestroy(s_h2d);
         if (s_d2h) cudaStreamDestroy(s_d2h);
         free_superchunk();
-        cudaFree(head_out);
     }
 
     void free_superchunk() {
         for (int i = 0; i < 2; ++i) {
-            if (sc_hin[i]) cudaFreeHost(sc_hin[i]);
-            if (sc_hout[i]) cudaFreeHost(sc_hout[i]);
-            cudaFree(sc_din[i]); cudaFree(sc_dout[i]);
+            sc_hin[i].reset(); sc_hout[i].reset();
+            sc_din[i] = DeviceBuffer(); sc_dout[i] = DeviceBuffer();
             if (sc_done[i]) cudaEventDestroy(sc_done[i]);
-            sc_hin[i] = sc_hout[i] = nullptr; sc_din[i] = sc_dout[i] = nullptr; sc_done[i] = nullptr;
+            sc_done[i] = nullptr;
             sc_pending[i] = false; sc_nout[i] = 0;
         }
         sc = 0; sc_fill = 0; sc_cur = 0;
@@ -98,12 +92,11 @@ struct Graph {
 
     int commit(int fuse) {
         stages.clear();
-        for (Block* b : fused) delete b;
         fused.clear();
         desc.clear();
         size_t i = 0;
         while (i < blocks.size()) {
-            Block* b = blocks[i];
+            Block* b = blocks[i].get();
             Block* st = b;
             Block* st2 = nullptr;        // a rewrite may turn a run of blocks into two stages
             size_t used = 1;
@@ -112,41 +105,38 @@ struct Graph {
                 FirBlock* fir = dynamic_cast<FirBlock*>(b);
                 IirBlock* iir = dynamic_cast<IirBlock*>(b);
                 if (rot && i + 1 < blocks.size()) {
-                    FirBlock* f2 = dynamic_cast<FirBlock*>(blocks[i + 1]);
-                    DownsampleBlock* d3 = (i + 2 < blocks.size()) ? dynamic_cast<DownsampleBlock*>(blocks[i + 2]) : nullptr;
+                    FirBlock* f2 = dynamic_cast<FirBlock*>(blocks[i + 1].get());
+                    DownsampleBlock* d3 = (i + 2 < blocks.size()) ? dynamic_cast<DownsampleBlock*>(blocks[i + 2].get()) : nullptr;
                     if (d3 && d3->in_size != 8) d3 = nullptr;
                     const bool fir_ok = f2 && (f2->kind == FIR_CRCF || f2->kind == FIR_CCCF) && f2->D == 1;
                     if (fir_ok && d3 && f2->kind == FIR_CRCF) {
-                        DiscrimBlock* d4 = (i + 3 < blocks.size()) ? dynamic_cast<DiscrimBlock*>(blocks[i + 3]) : nullptr;
-                        Block* t = make_tuner(rot->turns, (const float*)f2->h_taps.data(), f2->M, d3->D, d4 ? d4->gain : 0.0f);
-                        if (t) { fused.push_back(t); st = t; used = d4 ? 4 : 3; }
+                        DiscrimBlock* d4 = (i + 3 < blocks.size()) ? dynamic_cast<DiscrimBlock*>(blocks[i + 3].get()) : nullptr;
+                        std::unique_ptr<Block> t = make_tuner(rot->turns, (const float*)f2->h_taps.data(), f2->M, d3->D, d4 ? d4->gain : 0.0f);
+                        if (t) { st = t.get(); fused.push_back(std::move(t)); used = d4 ? 4 : 3; }
                     }
                     if (used == 1 && fir_ok && f2->M <= 513) {
                         // translator folded into the overlap-save kernel (any taps, complex taps included)
-                        FirBlock* nf = new (std::nothrow) FirBlock(f2->kind, f2->h_taps.data(), (unsigned)f2->M, (unsigned)(d3 ? d3->D : 1), true);
-                        if (!nf) { set_error("out of memory"); return -1; }
-                        nf->set_rotation(rot->turns);      // (the fused translator forces the overlap-save path: algo is moot)
-                        nf->name = f2->kind == FIR_CCCF ? "rot+fir_cccf" : "rot+fir_crcf";
-                        if (nf->init() != 0) { delete nf; return -1; }
-                        fused.push_back(nf); st = nf; used = d3 ? 3 : 2;
+                        auto nf = make_block<FirBlock>(f2->kind, f2->h_taps.data(), (unsigned)f2->M, (unsigned)(d3 ? d3->D : 1), true,
+                                                       true, rot->turns);
+                        if (!nf) return -1;
+                        st = nf.get(); fused.push_back(std::move(nf)); used = d3 ? 3 : 2;
                     }
                 }
                 {
                     // [MultiplyConstant(real c) ->] Upsampler(L) -> FIR(real taps) [-> Downsampler(D)]  =>  polyphase
                     // interpolating FIR (composites/interpolator.lua:31-41, composites/rationalresampler.lua:33-46)
                     size_t j = i;
-                    ScaleBlock* sc = dynamic_cast<ScaleBlock*>(blocks[j]);
+                    ScaleBlock* sc = dynamic_cast<ScaleBlock*>(blocks[j].get());
                     if (sc && !sc->complex_const) ++j; else sc = nullptr;
-                    UpsampleBlock* up = j < blocks.size() ? dynamic_cast<UpsampleBlock*>(blocks[j]) : nullptr;
-                    FirBlock* f2 = (up && j + 1 < blocks.size()) ? dynamic_cast<FirBlock*>(blocks[j + 1]) : nullptr;
+                    UpsampleBlock* up = j < blocks.size() ? dynamic_cast<UpsampleBlock*>(blocks[j].get()) : nullptr;
+                    FirBlock* f2 = (up && j + 1 < blocks.size()) ? dynamic_cast<FirBlock*>(blocks[j + 1].get()) : nullptr;
                     if (up && f2 && f2->D == 1 && (f2->kind == FIR_CRCF || f2->kind == FIR_RRRF) && f2->in_size == up->out_size) {
-                        DownsampleBlock* d3 = (j + 2 < blocks.size()) ? dynamic_cast<DownsampleBlock*>(blocks[j + 2]) : nullptr;
+                        DownsampleBlock* d3 = (j + 2 < blocks.size()) ? dynamic_cast<DownsampleBlock*>(blocks[j + 2].get()) : nullptr;
                         if (d3 && d3->in_size != f2->out_size) d3 = nullptr;
-                        InterpFirBlock* nb = new (std::nothrow) InterpFirBlock(f2->kind == FIR_CRCF, (const float*)f2->h_taps.data(), f2->M,
-                                                                               up->L, d3 ? d3->D : 1, sc != nullptr, sc ? sc->cre : 1.0f, true);
-                        if (!nb) { set_error("out of memory"); return -1; }
-                        if (nb->init() != 0) { delete nb; return -1; }
-                        fused.push_back(nb); st = nb; used = (j - i) + 2 + (d3 ? 1 : 0);
+                        auto nb = make_block<InterpFirBlock>(f2->kind == FIR_CRCF, (const float*)f2->h_taps.data(), f2->M, up->L,
+                                                             d3 ? d3->D : 1, sc != nullptr, sc ? sc->cre : 1.0f, true);
+                        if (!nb) return -1;
+                        st = nb.get(); fused.push_back(std::move(nb)); used = (j - i) + 2 + (d3 ? 1 : 0);
                     }
                 }
                 if (used == 1 && fir && fir->D == 1 && fir->kind == FIR_RRRF && i + 2 < blocks.size()) {
@@ -159,8 +149,8 @@ struct Graph {
                     // output rate, instead of a full-rate FIR and a full-rate recurrence that both compute D times more
                     // samples than the Downsampler keeps.  Zero initial state on both sides, so the streams are equal
                     // from the first sample; the taps are designed in float64 from the float32 coefficients.
-                    IirBlock* i2 = dynamic_cast<IirBlock*>(blocks[i + 1]);
-                    DownsampleBlock* d3 = dynamic_cast<DownsampleBlock*>(blocks[i + 2]);
+                    IirBlock* i2 = dynamic_cast<IirBlock*>(blocks[i + 1].get());
+                    DownsampleBlock* d3 = dynamic_cast<DownsampleBlock*>(blocks[i + 2].get());
                     if (i2 && !i2->complex_data && i2->D == 1 && d3 && d3->in_size == 4 && d3->D > 1) {
                         const int Dd = d3->D, nbb = i2->nb;
                         std::vector<double> g((size_t)(nbb + Dd - 1), 0.0);
@@ -178,51 +168,45 @@ struct Graph {
                                 if (t - k >= 0 && t - k < fir->M) acc += g[(size_t)k] * (double)h[t - k];
                             hc[(size_t)t] = (float)acc;
                         }
-                        FirBlock* nf = new (std::nothrow) FirBlock(FIR_RRRF, hc.data(), (unsigned)Mc, (unsigned)Dd, true);
-                        if (!nf) { set_error("out of memory"); return -1; }
+                        auto nf = make_block<FirBlock>(FIR_RRRF, hc.data(), (unsigned)Mc, (unsigned)Dd, true);
+                        if (!nf) return -1;
                         nf->set_algorithm(fir->algo);
-                        if (nf->init() != 0) { delete nf; return -1; }
                         if (nf->poly && nf->algo != LRB200_FIR_FFT && polyphase_pole_ok((float)cp)) {
                             // the pole's memory (|c^D|^64 <= 1e-8) fits the kernel's own warm-up: ONE stage
-                            if (nf->set_pole((float)cp) != 0) { delete nf; return -1; }
+                            if (nf->set_pole((float)cp) != 0) return -1;
                             nf->label = "fir*iir1_rrrf(" + std::to_string(Mc) + ",/" + std::to_string(Dd) + ")+pole";
                             nf->name = nf->label.c_str();
-                            fused.push_back(nf);
-                            st = nf; used = 3;
+                            st = nf.get(); used = 3;
+                            fused.push_back(std::move(nf));
                         } else if (nf->poly) {      // only worth it when the polyphase kernel has this shape
                             const float one = 1.0f, a2[2] = {1.0f, (float)(-cp)};     // cp == c^D
-                            IirBlock* ni = new (std::nothrow) IirBlock(false, &one, 1, a2, 2, true);
-                            if (!ni) { delete nf; set_error("out of memory"); return -1; }
-                            if (ni->init() != 0) { delete nf; delete ni; return -1; }
+                            auto ni = make_block<IirBlock>(false, &one, 1u, a2, 2u, true);
+                            if (!ni) return -1;
                             nf->label = "fir*iir1_rrrf(" + std::to_string(Mc) + ",/" + std::to_string(Dd) + ")";
                             nf->name = nf->label.c_str();
                             ni->name = "pole_rrrf";
-                            fused.push_back(nf); fused.push_back(ni);
-                            st = nf; st2 = ni; used = 3;
-                        } else {
-                            delete nf;
+                            st = nf.get(); st2 = ni.get(); used = 3;
+                            fused.push_back(std::move(nf)); fused.push_back(std::move(ni));
                         }
                     }
                 }
                 if (used == 1 && fir && fir->D == 1 && fir->kind != FIR_HILBERT && i + 1 < blocks.size()) {
-                    DownsampleBlock* d2 = dynamic_cast<DownsampleBlock*>(blocks[i + 1]);
+                    DownsampleBlock* d2 = dynamic_cast<DownsampleBlock*>(blocks[i + 1].get());
                     if (d2 && d2->in_size == fir->out_size) {
-                        FirBlock* nf = new (std::nothrow) FirBlock(fir->kind, fir->h_taps.data(), (unsigned)fir->M, (unsigned)d2->D, true);
-                        if (!nf) { set_error("out of memory"); return -1; }
+                        auto nf = make_block<FirBlock>(fir->kind, fir->h_taps.data(), (unsigned)fir->M, (unsigned)d2->D, true);
+                        if (!nf) return -1;
                         nf->set_algorithm(fir->algo);      // FIRFilterBlock(taps, use_fft) survives the fusion
-                        if (nf->init() != 0) { delete nf; return -1; }
-                        fused.push_back(nf); st = nf; used = 2;
+                        st = nf.get(); fused.push_back(std::move(nf)); used = 2;
                     }
                 }
                 if (used == 1 && iir && iir->D == 1 && i + 1 < blocks.size()) {
-                    DownsampleBlock* d2 = dynamic_cast<DownsampleBlock*>(blocks[i + 1]);
+                    DownsampleBlock* d2 = dynamic_cast<DownsampleBlock*>(blocks[i + 1].get());
                     if (d2 && d2->in_size == iir->out_size) {
                         float a[2] = {1.0f, -iir->c};
-                        IirBlock* ni = new (std::nothrow) IirBlock(iir->complex_data, iir->b, (unsigned)iir->nb, a, 2, true);
-                        if (!ni) { set_error("out of memory"); return -1; }
+                        auto ni = make_block<IirBlock>(iir->complex_data, iir->b, (unsigned)iir->nb, a, 2u, true);
+                        if (!ni) return -1;
                         ni->D = d2->D;
-                        if (ni->init() != 0) { delete ni; return -1; }
-                        fused.push_back(ni); st = ni; used = 2;
+                        st = ni.get(); fused.push_back(std::move(ni)); used = 2;
                     }
                 }
             }
@@ -254,16 +238,16 @@ struct Graph {
             m = stages[k]->max_output(m);
             size_t bytes = (m ? m : 1) * stages[k]->out_size;
             int slot = (int)(k & 1);
-            if (bytes > ring_cap[slot]) {
+            if (bytes > ring[slot].capacity()) {
                 // a stage still in flight may be reading the old buffer
                 LRB_CHECK(cudaStreamSynchronize(s));
-                if (Block::reserve(&ring[slot], &ring_cap[slot], bytes) != 0) return -1;
+                if (ring[slot].reserve(bytes) != 0) return -1;
             }
         }
         const void* in = dx;
         size_t cnt = n;
         for (size_t k = 0; k < stages.size(); ++k) {
-            void* out = (k + 1 == stages.size()) ? dy : ring[k & 1];
+            void* out = (k + 1 == stages.size()) ? dy : ring[k & 1].get();
             size_t no = 0;
             if (timing) {
                 if (tcount.size() < stages.size()) { tev.resize(stages.size()); tcount.assign(stages.size(), 0); }
@@ -301,15 +285,14 @@ struct Graph {
             // one chunk (every call of the reference's per-vector regime, pipe.lua:73): copy, kernels and copy back in
             // order on ONE stream with ONE synchronize -- no cross-stream events, nothing to overlap anyway
             const size_t mo = max_output(n);
-            if (n * isz > d_in_cap[0] || (mo ? mo : 1) * osz > d_out_cap[0]) {
+            if (n * isz > d_in[0].capacity() || (mo ? mo : 1) * osz > d_out[0].capacity()) {
                 LRB_CHECK(cudaStreamSynchronize(s));
-                if (Block::reserve(&d_in[0], &d_in_cap[0], (n ? n : 1) * isz) != 0) return -1;
-                if (Block::reserve(&d_out[0], &d_out_cap[0], (mo ? mo : 1) * osz) != 0) return -1;
+                if (d_in[0].reserve((n ? n : 1) * isz) != 0 || d_out[0].reserve((mo ? mo : 1) * osz) != 0) return -1;
             }
             size_t no = 0;
-            if (n) LRB_CHECK(cudaMemcpyAsync(d_in[0], x, n * isz, cudaMemcpyHostToDevice, s));
-            if (run_device(d_in[0], n, d_out[0], &no, s) != 0) return -1;
-            if (no) LRB_CHECK(cudaMemcpyAsync(y, d_out[0], no * osz, cudaMemcpyDeviceToHost, s));
+            if (n) LRB_CHECK(cudaMemcpyAsync(d_in[0].get(), x, n * isz, cudaMemcpyHostToDevice, s));
+            if (run_device(d_in[0].get(), n, d_out[0].get(), &no, s) != 0) return -1;
+            if (no) LRB_CHECK(cudaMemcpyAsync(y, d_out[0].get(), no * osz, cudaMemcpyDeviceToHost, s));
             LRB_CHECK(cudaStreamSynchronize(s));
             *n_out = no;
             return 0;
@@ -321,21 +304,20 @@ struct Graph {
             const int slot = it & 1;
             size_t nc = n - done < host_chunk ? n - done : host_chunk;
             size_t mo = max_output(nc);
-            if (nc * isz > d_in_cap[slot] || (mo ? mo : 1) * osz > d_out_cap[slot]) {
+            if (nc * isz > d_in[slot].capacity() || (mo ? mo : 1) * osz > d_out[slot].capacity()) {
                 LRB_CHECK(cudaDeviceSynchronize());
-                if (Block::reserve(&d_in[slot], &d_in_cap[slot], nc * isz) != 0) return -1;
-                if (Block::reserve(&d_out[slot], &d_out_cap[slot], (mo ? mo : 1) * osz) != 0) return -1;
+                if (d_in[slot].reserve(nc * isz) != 0 || d_out[slot].reserve((mo ? mo : 1) * osz) != 0) return -1;
             }
             if (it >= 2) LRB_CHECK(cudaStreamWaitEvent(s_h2d, ev_comp[slot], 0));     // d_in[slot] free again
-            LRB_CHECK(cudaMemcpyAsync(d_in[slot], (const char*)x + done * isz, nc * isz, cudaMemcpyHostToDevice, s_h2d));
+            LRB_CHECK(cudaMemcpyAsync(d_in[slot].get(), (const char*)x + done * isz, nc * isz, cudaMemcpyHostToDevice, s_h2d));
             LRB_CHECK(cudaEventRecord(ev_h2d[slot], s_h2d));
             LRB_CHECK(cudaStreamWaitEvent(s, ev_h2d[slot], 0));
             if (it >= 2) LRB_CHECK(cudaStreamWaitEvent(s, ev_d2h[slot], 0));          // d_out[slot] drained
             size_t no = 0;
-            if (run_device(d_in[slot], nc, d_out[slot], &no, s) != 0) return -1;
+            if (run_device(d_in[slot].get(), nc, d_out[slot].get(), &no, s) != 0) return -1;
             LRB_CHECK(cudaEventRecord(ev_comp[slot], s));
             LRB_CHECK(cudaStreamWaitEvent(s_d2h, ev_comp[slot], 0));
-            if (no) LRB_CHECK(cudaMemcpyAsync((char*)y + produced * osz, d_out[slot], no * osz, cudaMemcpyDeviceToHost, s_d2h));
+            if (no) LRB_CHECK(cudaMemcpyAsync((char*)y + produced * osz, d_out[slot].get(), no * osz, cudaMemcpyDeviceToHost, s_d2h));
             LRB_CHECK(cudaEventRecord(ev_d2h[slot], s_d2h));
             produced += no;
             done += nc;
@@ -358,10 +340,12 @@ struct Graph {
         const size_t isz = stages.front()->in_size, osz = stages.back()->out_size;
         sc_outcap = max_output(samples) + 1;
         for (int i = 0; i < 2; ++i) {
-            LRB_CHECK(cudaHostAlloc((void**)&sc_hin[i], samples * isz, cudaHostAllocDefault));
-            LRB_CHECK(cudaHostAlloc((void**)&sc_hout[i], sc_outcap * osz, cudaHostAllocDefault));
-            LRB_CHECK(cudaMalloc(&sc_din[i], samples * isz));
-            LRB_CHECK(cudaMalloc(&sc_dout[i], sc_outcap * osz));
+            char* p = nullptr;
+            LRB_CHECK(cudaHostAlloc((void**)&p, samples * isz, cudaHostAllocDefault));
+            sc_hin[i].reset(p);
+            LRB_CHECK(cudaHostAlloc((void**)&p, sc_outcap * osz, cudaHostAllocDefault));
+            sc_hout[i].reset(p);
+            if (sc_din[i].reserve(samples * isz) != 0 || sc_dout[i].reserve(sc_outcap * osz) != 0) return -1;
             LRB_CHECK(cudaEventCreateWithFlags(&sc_done[i], cudaEventDisableTiming));
         }
         sc = samples;
@@ -371,7 +355,7 @@ struct Graph {
         if (!sc_pending[slot]) return 0;
         if (!cuda_ok(cudaEventSynchronize(sc_done[slot]), "cudaEventSynchronize")) return (size_t)-1;
         const size_t osz = stages.back()->out_size;
-        if (sc_nout[slot]) memcpy(y, sc_hout[slot], sc_nout[slot] * osz);
+        if (sc_nout[slot]) memcpy(y, sc_hout[slot].get(), sc_nout[slot] * osz);
         sc_pending[slot] = false;
         return sc_nout[slot];
     }
@@ -379,9 +363,9 @@ struct Graph {
         cudaStream_t s = ctx().stream;
         const size_t isz = stages.front()->in_size, osz = stages.back()->out_size;
         size_t no = 0;
-        LRB_CHECK(cudaMemcpyAsync(sc_din[slot], sc_hin[slot], count * isz, cudaMemcpyHostToDevice, s));
-        if (run_device(sc_din[slot], count, sc_dout[slot], &no, s) != 0) return -1;
-        if (no) LRB_CHECK(cudaMemcpyAsync(sc_hout[slot], sc_dout[slot], no * osz, cudaMemcpyDeviceToHost, s));
+        LRB_CHECK(cudaMemcpyAsync(sc_din[slot].get(), sc_hin[slot].get(), count * isz, cudaMemcpyHostToDevice, s));
+        if (run_device(sc_din[slot].get(), count, sc_dout[slot].get(), &no, s) != 0) return -1;
+        if (no) LRB_CHECK(cudaMemcpyAsync(sc_hout[slot].get(), sc_dout[slot].get(), no * osz, cudaMemcpyDeviceToHost, s));
         LRB_CHECK(cudaEventRecord(sc_done[slot], s));
         sc_nout[slot] = no;
         sc_pending[slot] = true;
@@ -394,7 +378,7 @@ struct Graph {
         size_t produced = 0;
         while (n > 0) {
             const size_t take = n < sc - sc_fill ? n : sc - sc_fill;
-            memcpy(sc_hin[sc_cur] + sc_fill * isz, xp, take * isz);
+            memcpy(sc_hin[sc_cur].get() + sc_fill * isz, xp, take * isz);
             sc_fill += take; xp += take * isz; n -= take;
             if (sc_fill == sc) {
                 // the other slot was submitted one super-chunk ago: its results are (long) ready
@@ -429,14 +413,16 @@ struct Graph {
         return 0;
     }
 
+    // Block::reset for every block, with ONE launch zeroing the carried state of them all
     int reset(cudaStream_t s) {
-        std::vector<std::pair<void*, size_t>> segs;
-        for (Block* b : blocks) { b->reset_host(); b->state_buffers(segs); }
-        for (Block* b : fused) { b->reset_host(); b->state_buffers(segs); }
-        if (segs.empty()) return 0;
         std::vector<void*> ptrs;
         std::vector<size_t> bytes;
-        for (auto& sg : segs) { ptrs.push_back(sg.first); bytes.push_back(sg.second); }
+        for (auto* list : {&blocks, &fused})
+            for (auto& b : *list) {
+                b->rewind();
+                for (auto& sg : b->carried) { ptrs.push_back(sg.first); bytes.push_back(sg.second); }
+            }
+        if (ptrs.empty()) return 0;
         return launch_zero_segments(ptrs.data(), bytes.data(), (int)ptrs.size(), s);
     }
     int reset() { return reset(ctx().stream); }
@@ -515,9 +501,9 @@ struct Graph {
             lead[K] = (size_t)(b - a);                       // outputs of the halo: dropped
         }
         const size_t ho = lead[K];
-        if ((ho + 1) * osz > head_out_cap) {
+        if ((ho + 1) * osz > head_out.capacity()) {
             LRB_CHECK(cudaStreamSynchronize(s));
-            if (Block::reserve(&head_out, &head_out_cap, (ho + 1) * osz) != 0) return -1;
+            if (head_out.reserve((ho + 1) * osz) != 0) return -1;
         }
         // ring for halo + n inputs
         const size_t n_tot = halo_n + n;
@@ -526,9 +512,9 @@ struct Graph {
             m = stages[k]->max_output(m);
             const size_t bytes = (m ? m : 1) * stages[k]->out_size;
             const int slot = (int)(k & 1);
-            if (bytes > ring_cap[slot]) {
+            if (bytes > ring[slot].capacity()) {
                 LRB_CHECK(cudaStreamSynchronize(s));
-                if (Block::reserve(&ring[slot], &ring_cap[slot], bytes) != 0) return -1;
+                if (ring[slot].reserve(bytes) != 0) return -1;
             }
         }
         const bool overlap = halo_ready && K >= 2 && stages[0]->supports_lead_wait();
@@ -545,7 +531,7 @@ struct Graph {
             if (k == 0 && overlap) { ctx().lead_samples = (long long)halo_n; ctx().lead_event = halo_ready; ctx().reserve_ctas = 4; }
             size_t no = 0;
             if (!last) {
-                void* out = ring[k & 1];
+                void* out = ring[k & 1].get();
                 rc = stages[k]->run(in, cnt, out, &no, s);
                 in = out;
                 cnt = no;
@@ -556,7 +542,7 @@ struct Graph {
                 size_t no1 = 0;
                 const size_t m1 = lead[k] < cnt ? lead[k] : cnt;
                 cudaStream_t s1 = (stages[k]->state_only_on_side_stream() && cnt - m1 >= SIDE_STREAM_MIN) ? side_fork(s) : s;
-                rc = stages[k]->run(in, m1, head_out, &no1, s1);
+                rc = stages[k]->run(in, m1, head_out.get(), &no1, s1);
                 if (rc == 0 && no1 != ho) { set_error("graph: halo produced %zu outputs, expected %zu", no1, ho); rc = -1; }
                 if (rc == 0) rc = stages[k]->run((const char*)in + m1 * stages[k]->in_size, cnt - m1, dy, &no, s);
                 side_join(s, s1);
@@ -593,12 +579,12 @@ struct Graph {
 void destroy_graph_handle(void* holder);      // delete (lrb200_graph_t*) -- defined behind the handle type below
 
 struct DagNode {
-    Block* blk = nullptr;          // owned
+    std::unique_ptr<Block> blk;
     Graph* sub = nullptr;          // a committed linear run: lives inside `holder` (the caller's former handle, owned)
     void* holder = nullptr;
     std::vector<int> in_refs;      // producer node * 4 + port, or -1 for the DAG input
-    std::vector<void*> out_buf;
-    std::vector<size_t> out_cap, out_cnt;
+    std::vector<DeviceBuffer> out_buf;
+    std::vector<size_t> out_cnt;
     int nout() const { return sub ? 1 : blk->num_outputs; }
     size_t out_size(int port) const { return sub ? sub->stages.back()->out_size : blk->out_size_of(port); }
     size_t in_size() const { return sub ? sub->stages.front()->in_size : blk->in_size; }
@@ -608,23 +594,30 @@ struct DagNode {
 struct Dag {
     std::vector<DagNode> nodes;
     std::vector<int> outputs;
-    void* d_in = nullptr; size_t d_in_cap = 0;
+    DeviceBuffer d_in;
     size_t in_size = 0;
     std::string desc;
 
     ~Dag() {
-        for (DagNode& nd : nodes) {
-            delete nd.blk;
+        for (DagNode& nd : nodes)
             if (nd.holder) destroy_graph_handle(nd.holder);
-            for (void* p : nd.out_buf) cudaFree(p);
-        }
-        cudaFree(d_in);
     }
 
+    // on success the DAG owns blk (or holder); on failure the caller keeps it
     int add(Block* blk, Graph* sub, void* holder, const int* refs, unsigned nin) {
         DagNode nd;
-        nd.blk = blk; nd.sub = sub; nd.holder = holder;
-        const int want = sub ? 1 : blk->num_inputs;
+        nd.blk.reset(blk); nd.sub = sub; nd.holder = holder;
+        if (wire(nd, refs, nin) != 0) { nd.blk.release(); return -1; }
+        nd.out_buf.resize((size_t)nd.nout());
+        nd.out_cnt.assign((size_t)nd.nout(), 0);
+        if (!desc.empty()) desc += " ; ";
+        desc += nd.name();
+        nodes.push_back(std::move(nd));
+        return (int)nodes.size() - 1;
+    }
+
+    int wire(DagNode& nd, const int* refs, unsigned nin) {
+        const int want = nd.sub ? 1 : nd.blk->num_inputs;
         if ((int)nin != want) { set_error("dag: %s takes %d input(s), got %u", nd.name(), want, nin); return -1; }
         for (unsigned i = 0; i < nin; ++i) {
             const int r = refs[i];
@@ -641,13 +634,7 @@ struct Dag {
             if (esz != nd.in_size()) { set_error("dag: %zu-byte samples cannot feed %s (%zu-byte input)", esz, nd.name(), nd.in_size()); return -1; }
             nd.in_refs.push_back(r);
         }
-        nd.out_buf.assign((size_t)nd.nout(), nullptr);
-        nd.out_cap.assign((size_t)nd.nout(), 0);
-        nd.out_cnt.assign((size_t)nd.nout(), 0);
-        nodes.push_back(nd);
-        if (!desc.empty()) desc += " ; ";
-        desc += nd.name();
-        return (int)nodes.size() - 1;
+        return 0;
     }
 
     int reset() {
@@ -661,35 +648,38 @@ struct Dag {
     int run_host(const void* x, size_t n, void* const* y, size_t* n_out) {
         if (nodes.empty() || outputs.empty()) { set_error("dag: no nodes / no outputs"); return -1; }
         cudaStream_t s = ctx().stream;
-        if (n * in_size > d_in_cap) {
+        if (n * in_size > d_in.capacity()) {
             LRB_CHECK(cudaStreamSynchronize(s));
-            if (Block::reserve(&d_in, &d_in_cap, n * in_size) != 0) return -1;
+            if (d_in.reserve(n * in_size) != 0) return -1;
         }
-        if (n) LRB_CHECK(cudaMemcpyAsync(d_in, x, n * in_size, cudaMemcpyHostToDevice, s));
+        if (n) LRB_CHECK(cudaMemcpyAsync(d_in.get(), x, n * in_size, cudaMemcpyHostToDevice, s));
         for (DagNode& nd : nodes) {
             std::vector<const void*> ins;
             size_t cnt = 0;
             for (size_t i = 0; i < nd.in_refs.size(); ++i) {
                 const int r = nd.in_refs[i];
-                const void* p = r == -1 ? d_in : nodes[(size_t)(r >> 2)].out_buf[(size_t)(r & 3)];
+                const void* p = r == -1 ? d_in.get() : nodes[(size_t)(r >> 2)].out_buf[(size_t)(r & 3)].get();
                 const size_t c = r == -1 ? n : nodes[(size_t)(r >> 2)].out_cnt[(size_t)(r & 3)];
                 if (i && c != cnt) { set_error("dag: %s received inputs of different lengths (%zu, %zu)", nd.name(), cnt, c); return -1; }
                 cnt = c;
                 ins.push_back(p);
             }
             const size_t mo = nd.sub ? nd.sub->max_output(cnt) : nd.blk->max_output(cnt);
+            void* outs[4];                 // a port is two bits of a reference
             for (int o = 0; o < nd.nout(); ++o) {
+                DeviceBuffer& buf = nd.out_buf[(size_t)o];
                 const size_t bytes = (mo ? mo : 1) * nd.out_size(o);
-                if (bytes > nd.out_cap[(size_t)o]) {
+                if (bytes > buf.capacity()) {
                     LRB_CHECK(cudaStreamSynchronize(s));
-                    if (Block::reserve(&nd.out_buf[(size_t)o], &nd.out_cap[(size_t)o], bytes) != 0) return -1;
+                    if (buf.reserve(bytes) != 0) return -1;
                 }
+                outs[o] = buf.get();
             }
             size_t no = 0;
             if (nd.sub) {
-                if (nd.sub->run_device(ins[0], cnt, nd.out_buf[0], &no, s) != 0) return -1;
+                if (nd.sub->run_device(ins[0], cnt, outs[0], &no, s) != 0) return -1;
             } else {
-                if (nd.blk->run_multi(ins.data(), (int)ins.size(), cnt, nd.out_buf.data(), nd.nout(), &no, s) != 0) return -1;
+                if (nd.blk->run_multi(ins.data(), (int)ins.size(), cnt, outs, nd.nout(), &no, s) != 0) return -1;
             }
             for (int o = 0; o < nd.nout(); ++o) nd.out_cnt[(size_t)o] = no;
         }
@@ -697,7 +687,7 @@ struct Dag {
             const DagNode& nd = nodes[(size_t)(outputs[k] >> 2)];
             const int port = outputs[k] & 3;
             const size_t c = nd.out_cnt[(size_t)port];
-            if (c) LRB_CHECK(cudaMemcpyAsync(y[k], nd.out_buf[(size_t)port], c * nd.out_size(port), cudaMemcpyDeviceToHost, s));
+            if (c) LRB_CHECK(cudaMemcpyAsync(y[k], nd.out_buf[(size_t)port].get(), c * nd.out_size(port), cudaMemcpyDeviceToHost, s));
             n_out[k] = c;
         }
         LRB_CHECK(cudaStreamSynchronize(s));
@@ -731,7 +721,7 @@ int lrb200_graph_append(lrb200_graph_t* g, lrb200_block_t* q) {
                   g->g.blocks.back()->out_size, q->impl->name, q->impl->in_size);
         return -1;
     }
-    g->g.blocks.push_back(q->impl);
+    g->g.blocks.emplace_back(q->impl);
     g->g.committed = false;
     q->impl = nullptr;          // ownership moves to the graph
     delete q;

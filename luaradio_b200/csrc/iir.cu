@@ -340,18 +340,11 @@ next_tile:
 
 int iir_work_alloc(IirScanWork* w, int elem_size) {
     w->max_tiles = 1 << 15;   // 128 Mi samples per launch
-    LRB_CHECK(cudaMalloc(&w->ticket, sizeof(int)));
-    LRB_CHECK(cudaMalloc(&w->flags, sizeof(int) * w->max_tiles));
-    LRB_CHECK(cudaMalloc(&w->agg, (size_t)elem_size * w->max_tiles));
-    LRB_CHECK(cudaMalloc(&w->pfx, (size_t)elem_size * w->max_tiles));
-    LRB_CHECK(cudaMemset(w->flags, 0, sizeof(int) * w->max_tiles));
+    if (w->ticket.reserve(sizeof(int)) != 0 || w->flags.alloc_zeroed(sizeof(int) * w->max_tiles) != 0 ||
+        w->agg.reserve((size_t)elem_size * w->max_tiles) != 0 || w->pfx.reserve((size_t)elem_size * w->max_tiles) != 0)
+        return -1;
     w->epoch = 0;
     return 0;
-}
-
-void iir_work_free(IirScanWork* w) {
-    cudaFree(w->ticket); cudaFree(w->flags); cudaFree(w->agg); cudaFree(w->pfx);
-    *w = IirScanWork();
 }
 
 long long iir_max_per_launch(const IirScanWork& w) { return (long long)w.max_tiles * IIR_TILE; }
@@ -386,14 +379,14 @@ int launch_iir1(bool complex_data, const void* x, long long n, void* y, const fl
     }
     w->epoch = (w->epoch + 1) & 0x3fffffffu;
     if (w->epoch == 0) {                          // wrapped: clear stale flags
-        LRB_CHECK(cudaMemsetAsync(w->flags, 0, sizeof(int) * w->max_tiles, s));
+        LRB_CHECK(cudaMemsetAsync(w->flags.get(), 0, sizeof(int) * w->max_tiles, s));
         w->epoch = 1;
     }
-    LRB_CHECK(cudaMemsetAsync(w->ticket, 0, sizeof(int), s));
+    LRB_CHECK(cudaMemsetAsync(w->ticket.get(), 0, sizeof(int), s));
     int tiles = (int)((n + IIR_TILE - 1) / IIR_TILE);
 #define LRB_IIR_SCAN(TT, NN)                                                                                    \
     iir1_scan_kernel<TT, false, NN><<<tiles, IIR_THREADS, 0, s>>>((const TT*)x, n, (TT*)y, P, (const TT*)xhist_in,  \
-        (TT*)xhist_out, (const TT*)ystate_in, (TT*)ystate_out, first, D, w->ticket, w->flags, (TT*)w->agg, (TT*)w->pfx, w->epoch)
+        (TT*)xhist_out, (const TT*)ystate_in, (TT*)ystate_out, first, D, w->ticket.as<int>(), w->flags.as<int>(), w->agg.as<TT>(), w->pfx.as<TT>(), w->epoch)
     if (complex_data) { if (nb == 2) LRB_IIR_SCAN(float2, 2); else if (nb == 1) LRB_IIR_SCAN(float2, 1); else LRB_IIR_SCAN(float2, IIR_MAX_NB); }
     else { if (nb == 2) LRB_IIR_SCAN(float, 2); else if (nb == 1) LRB_IIR_SCAN(float, 1); else LRB_IIR_SCAN(float, IIR_MAX_NB); }
 #undef LRB_IIR_SCAN

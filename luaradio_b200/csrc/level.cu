@@ -368,46 +368,26 @@ LevelBlock::LevelBlock(bool agc_, double power_alpha, double gain_alpha, double 
     theta = threshold;
 }
 
-LevelBlock::~LevelBlock() {
-    cudaFree(d_state[0]); cudaFree(d_state[1]);
-    cudaFree(d_pw); cudaFree(d_ticket); cudaFree(d_rec);
-}
-
 int LevelBlock::init() {
-    for (int i = 0; i < 2; ++i) {
-        LRB_CHECK(cudaMalloc(&d_state[i], 2 * sizeof(double)));
-        LRB_CHECK(cudaMemset(d_state[i], 0, 2 * sizeof(double)));
-    }
-    LRB_CHECK(cudaMalloc(&d_ticket, sizeof(unsigned long long)));
-    LRB_CHECK(cudaMemset(d_ticket, 0, sizeof(unsigned long long)));
-    LRB_CHECK(cudaMalloc(&d_rec, rec_bytes()));
-    LRB_CHECK(cudaMemset(d_rec, 0, rec_bytes()));
+    if (carry(d_state, 2 * sizeof(double), cur) != 0 || d_ticket.alloc_zeroed(sizeof(unsigned long long)) != 0 ||
+        d_rec.alloc_zeroed(rec_bytes()) != 0)
+        return -1;
     if (agc) {
         // b^k for the in-tile compositions (k <= one tile's samples)
         std::vector<double> pw((size_t)LV_TILE + 1);
         const double b = 1 - ga;
         pw[0] = 1.0;
         for (int k = 1; k <= LV_TILE; ++k) pw[(size_t)k] = pw[(size_t)k - 1] * b;
-        LRB_CHECK(cudaMalloc(&d_pw, sizeof(double) * pw.size()));
-        LRB_CHECK(cudaMemcpy(d_pw, pw.data(), sizeof(double) * pw.size(), cudaMemcpyHostToDevice));
+        if (d_pw.upload(pw.data(), sizeof(double) * pw.size()) != 0) return -1;
     }
     return 0;
-}
-
-void LevelBlock::reset_host() { consumed = 0; cur = 0; }
-
-void LevelBlock::state_buffers(std::vector<std::pair<void*, size_t>>& segs) {
-    segs.push_back({d_state[0], 2 * sizeof(double)});
-    segs.push_back({d_state[1], 2 * sizeof(double)});
 }
 
 long long LevelBlock::memory_in() const {
     if (agc) return -1;                    // a closed gate holds the gain for ever
     // the power estimator's pole decays to 1e-12 (as IirBlock::memory_in)
-    const double a = std::fabs(1 - pa);
-    if (a == 0.0) return 1;
-    if (a >= 1.0) return -1;
-    return (long long)std::ceil(std::log(1e-12) / std::log(a)) + 2;
+    const long long w = decay_samples(1 - pa);
+    return w < 0 ? -1 : w + 1;
 }
 
 int LevelBlock::run(const void* dx, size_t n, void* dy, size_t* n_out, cudaStream_t s) {
@@ -425,25 +405,25 @@ int LevelBlock::run(const void* dx, size_t n, void* dy, size_t* n_out, cudaStrea
     double q = P.b;
     for (int k = 0; k < 32; ++k) { P.b2[k] = q; q = q * q; }
     LevelRecords R;
-    R.ticket = (unsigned long long*)d_ticket;
-    R.rec_a = (uint4*)d_rec;
-    R.rec_b = agc ? (uint4*)d_rec + LEVEL_MAX_TILES : nullptr;
+    R.ticket = d_ticket.as<unsigned long long>();
+    R.rec_a = d_rec.as<uint4>();
+    R.rec_b = agc ? d_rec.as<uint4>() + LEVEL_MAX_TILES : nullptr;
     const long long maxn = (long long)LEVEL_MAX_TILES * LV_TILE;
     size_t done = 0;
     while (done < n) {
         const long long nc = (long long)(n - done) < maxn ? (long long)(n - done) : maxn;
         epoch = (epoch + 1) & 0x3fffffffu;
         if (epoch == 0) {                  // wrapped: clear stale flags
-            LRB_CHECK(cudaMemsetAsync(d_rec, 0, rec_bytes(), s));
+            LRB_CHECK(cudaMemsetAsync(d_rec.get(), 0, rec_bytes(), s));
             epoch = 1;
         }
         const int tiles = (int)((nc + LV_TILE - 1) / LV_TILE);
         const char* xin = (const char*)dx + done * in_size;
         char* yout = (char*)dy + done * out_size;
-        const double2* si = (const double2*)d_state[cur];
-        double2* so = (double2*)d_state[cur ^ 1];
+        const double2* si = d_state[cur].as<const double2>();
+        double2* so = d_state[cur ^ 1].as<double2>();
 #define LRB_LEVEL(TT, AA)                                                                                           \
-        level_kernel<TT, AA><<<tiles, LV_THREADS, 0, s>>>((const TT*)xin, nc, (TT*)yout, P, d_pw, si, so, R, ticket_base, epoch)
+        level_kernel<TT, AA><<<tiles, LV_THREADS, 0, s>>>((const TT*)xin, nc, (TT*)yout, P, d_pw.as<double>(), si, so, R, ticket_base, epoch)
         if (complex_data) { if (agc) LRB_LEVEL(float2, true); else LRB_LEVEL(float2, false); }
         else { if (agc) LRB_LEVEL(float, true); else LRB_LEVEL(float, false); }
 #undef LRB_LEVEL

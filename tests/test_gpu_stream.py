@@ -459,3 +459,169 @@ def test_wbfm_mono_chain_reference_executed_golden_fused(chunk):
     assert len(got) == len(g["y"]), (len(got), len(g["y"]))
     d = np.abs(got - g["y"])
     assert float(d.max()) <= 1e-5, "max |fused - reference| = %.3g at output %d of %d (graph %s)" % (float(d.max()), int(d.argmax()), len(d), top.describe_gpu_graph())
+
+
+# ---- reset: every block kind with carried state ------------------------------------------------------------------------
+# Each case runs x, then part of x (leaving state behind), resets, runs x again: the second full run must be bit-identical
+# to the first.  Blocks go through lrb200_block_reset, graph-only fused stages through lrb200_graph_reset, a device DAG
+# through lrb200_dag_reset.
+N_RESET, PART = 100003, 12345
+
+
+def _fir(kind, algo, decim):
+    def create(lib):
+        taps = np.linspace(-1, 1, 33, dtype=np.float32) * np.hamming(33).astype(np.float32)
+        if kind == "cccf":
+            taps = (taps + 0.5j * taps[::-1]).astype(np.complex64)
+        h = getattr(lib, "lrb200_fir_create_" + kind)(taps.ctypes.data, len(taps), decim, _lib.LRB200_HOST)
+        _lib.check(lib.lrb200_fir_set_algorithm(_lib.check_handle(h, "fir"), algo))
+        return h
+    return create, kind == "rrrf", 1
+
+
+def _iir(cplx, order):
+    def create(lib):
+        import scipy.signal
+        b, a = scipy.signal.butter(order, 0.1)
+        b, a = b.astype(np.float32), a.astype(np.float32)
+        return getattr(lib, "lrb200_iir_create_" + ("crcf" if cplx else "rrrf"))(b.ctypes.data, len(b), a.ctypes.data, len(a), _lib.LRB200_HOST)
+    return create, not cplx, 1
+
+
+HILBERT_TAPS = np.hamming(33).astype(np.float32)
+BLOCK_RESET_CASES = {
+    **{"fir_%s_%s_d%d" % (k, a, d): _fir(k, algo, d) for k in ("crcf", "cccf", "rrrf")
+       for a, algo in (("direct", _lib.FIR_DIRECT), ("fft", _lib.FIR_FFT)) for d in (1, 3)},
+    "hilbert": (lambda lib: lib.lrb200_hilbert_create(HILBERT_TAPS.ctypes.data, len(HILBERT_TAPS), _lib.LRB200_HOST), True, 1),
+    "translator": (lambda lib: lib.lrb200_rotator_create(0.0123, _lib.LRB200_HOST), False, 1),
+    "discriminator": (lambda lib: lib.lrb200_discrim_create(1.25, _lib.LRB200_HOST), False, 1),
+    "iir_singlepole_rrrf": _iir(False, 1),
+    "iir_singlepole_crcf": _iir(True, 1),
+    "iir_general_rrrf": _iir(False, 4),
+    "iir_general_crcf": _iir(True, 4),
+    "delay": (lambda lib: lib.lrb200_delay_create(100, 8, _lib.LRB200_HOST), False, 1),
+    "pll": (lambda lib: lib.lrb200_pll_create(1000.0, -2e3, 2e3, 2.0, 1e5, _lib.LRB200_HOST), False, 2),
+    # AGCBlock('custom', -20, -40, {gain_tau = 1e-3, power_tau = 5e-5}) and PowerSquelchBlock(-45) at 1 MHz, complex
+    "agc": (lambda lib: lib.lrb200_agc_create(-20.0, -40.0, 1e-3, 5e-5, 1e6, 1, _lib.LRB200_HOST), "bursty", 1),
+    "powersquelch": (lambda lib: lib.lrb200_powersquelch_create(-45.0, 1e-3, 1e6, 1, _lib.LRB200_HOST), "bursty", 1),
+}
+
+
+def _reset_input(real):
+    if real == "bursty":             # the level blocks' gate opens and closes inside tiles, on tile edges and for whole tiles
+        from tests.test_gpu_level import bursty_stream
+        return bursty_stream(1 << 20, True, 3)
+    rng = np.random.default_rng(21)
+    t = np.arange(N_RESET)
+    x = (np.exp(2j * np.pi * 0.003 * t) * (0.1 + 0.1 * (t % 20000 < 9000)) + 0.01 * rnd_c(rng, N_RESET)).astype(np.complex64)
+    return np.ascontiguousarray(x.real) if real else x
+
+
+def _run_ports(lib, h, x, nout):
+    cap = lib.lrb200_block_max_output(h, len(x))
+    outs = [np.zeros(cap * 8, np.uint8) for _ in range(nout)]
+    ins = (ctypes.c_void_p * 1)(x.ctypes.data)
+    ptrs = (ctypes.c_void_p * nout)(*[o.ctypes.data for o in outs])
+    no = ctypes.c_size_t()
+    _lib.check(lib.lrb200_block_execute_multi(h, ins, 1, len(x), ptrs, nout, ctypes.byref(no)), "execute")
+    return [o[:no.value * lib.lrb200_block_out_size(h) if k == 0 else no.value * 4] for k, o in enumerate(outs)]
+
+
+@pytest.mark.parametrize("case", list(BLOCK_RESET_CASES))
+def test_block_reset_restores_the_initial_state(case):
+    lib = _lib.require_device()
+    create, real, nout = BLOCK_RESET_CASES[case]
+    h = _lib.check_handle(create(lib), case)
+    try:
+        x = _reset_input(real)
+        first = _run_ports(lib, h, x, nout)
+        _run_ports(lib, h, x[:PART], nout)
+        _lib.check(lib.lrb200_block_reset(h), "reset")
+        again = _run_ports(lib, h, x, nout)
+        assert len(first[0]) > 0
+        for a, b in zip(first, again):
+            assert np.array_equal(a, b), case
+    finally:
+        lib.lrb200_block_destroy(h)
+
+
+def _audio_tail(rate):
+    # FIR -> de-emphasis -> /5: one stage with the pole fused when c^5 decays fast enough (low rate), else FIR | pole
+    return [mk(radio.LowpassFilterBlock, (128, 15e3), Float32, rate), mk(radio.FMDeemphasisFilterBlock, (75e-6,), Float32, rate),
+            mk(radio.DownsamplerBlock, (5,), Float32, rate)]
+
+
+GRAPH_RESET_CASES = {
+    "tuner+discrim": (lambda: [mk(radio.FrequencyTranslatorBlock, (-1e5,), ComplexFloat32, 1e6),
+                               mk(radio.LowpassFilterBlock, (128, 1e5), ComplexFloat32, 1e6),
+                               mk(radio.DownsamplerBlock, (5,), ComplexFloat32, 1e6),
+                               mk(radio.FrequencyDiscriminatorBlock, (1.25,), ComplexFloat32, 1e6)], False, np.float32, "tuner+discrim("),
+    "fir*iir1_rrrf+pole": (lambda: _audio_tail(1e5), True, np.float32, ")+pole"),
+    "fir*iir1_rrrf|pole_rrrf": (lambda: _audio_tail(1e6), True, np.float32, " | pole_rrrf"),
+    "resampler": (lambda: [mk(radio.UpsamplerBlock, (3,), ComplexFloat32, 1e6),
+                           mk(radio.LowpassFilterBlock, (64, 1e5), ComplexFloat32, 3e6),
+                           mk(radio.DownsamplerBlock, (2,), ComplexFloat32, 3e6)], False, np.complex64, "upsample+fir+down("),
+    "interpolator": (lambda: [mk(radio.UpsamplerBlock, (4,), Float32, 1e6),
+                              mk(radio.LowpassFilterBlock, (64, 1e5), Float32, 4e6)], True, np.float32, "upsample+fir("),
+    "iir/D": (lambda: [mk(radio.SinglepoleLowpassFilterBlock, (1e4,), ComplexFloat32, 1e6),
+                       mk(radio.DownsamplerBlock, (4,), ComplexFloat32, 1e6)], False, np.complex64, "iir_crcf[fused x2]"),
+}
+
+
+@pytest.mark.parametrize("case", list(GRAPH_RESET_CASES))
+def test_graph_reset_restores_the_initial_state(case):
+    lib = _lib.require_device()
+    make_blocks, real, out_dtype, fused_name = GRAPH_RESET_CASES[case]
+    g = _lib.check_handle(lib.lrb200_graph_create(), "graph")
+    try:
+        for b in make_blocks():
+            _lib.check(lib.lrb200_graph_append(g, b.make_device_handle()), "append")
+        _lib.check(lib.lrb200_graph_commit(g, 1), "commit")
+        assert fused_name in lib.lrb200_graph_describe(g).decode(), lib.lrb200_graph_describe(g)
+        x = _reset_input(real)
+
+        def run(v):
+            y = np.zeros(lib.lrb200_graph_max_output(g, len(v)), out_dtype)
+            no = ctypes.c_size_t()
+            _lib.check(lib.lrb200_graph_execute(g, v.ctypes.data, len(v), y.ctypes.data, ctypes.byref(no)), "execute")
+            return y[:no.value]
+        first = run(x)
+        run(x[:PART])
+        _lib.check(lib.lrb200_graph_reset(g), "graph_reset")
+        assert len(first) > 0 and np.array_equal(run(x).view(np.uint32), first.view(np.uint32))
+    finally:
+        lib.lrb200_graph_destroy(g)
+
+
+def test_dag_reset_restores_the_initial_state():
+    """The WBFM-stereo demodulator as one device DAG (PLL, delay, fused FIR runs, binary blocks, de-emphasis)."""
+    from luaradio_b200.composite import GPUDagBlock
+    lib = _lib.require_device()
+    rate, n = 220500.0, 60000
+    t = np.arange(n) / rate
+    mpx = 0.4 * np.sin(2 * np.pi * 700 * t) + 0.1 * np.sin(2 * np.pi * 19e3 * t) + 0.3 * np.sin(2 * np.pi * 2300 * t) * np.sin(2 * np.pi * 38e3 * t)
+    x = np.exp(2j * np.pi * 75e3 * np.cumsum(mpx) / rate).astype(np.complex64)
+    top = radio.CompositeBlock()
+    demod = radio.WBFMStereoDemodulator()
+    top.connect(radio.ArraySource(x, rate, n), demod)
+    top.connect(demod, "left", radio.ArraySink(), "in")
+    top.connect(demod, "right", radio.ArraySink(), "in")
+    top._prepare_to_run()
+    top._collapse_gpu_runs(True, 0, True)
+    dags = [c for c in top._chains if isinstance(c, GPUDagBlock)]
+    try:
+        assert len(dags) == 1
+        dag = dags[0]
+
+        def run(v):
+            return [np.array(o.data, copy=True) for o in dag.process(Vector.cast(v))]
+        first = run(x)
+        run(x[:PART])
+        _lib.check(lib.lrb200_dag_reset(dag.dag), "dag_reset")
+        again = run(x)
+        assert len(first[0]) == n
+        for a, b in zip(first, again):
+            assert np.array_equal(a.view(np.uint32), b.view(np.uint32))
+    finally:
+        for c in top._chains:
+            c.cleanup()
