@@ -221,6 +221,17 @@ lrb200_block_t* lrb200_agc_create(double target_dbfs, double threshold_dbfs, dou
                                   unsigned complex_data, unsigned flags);
 lrb200_block_t* lrb200_powersquelch_create(double threshold_dbfs, double tau, double rate, unsigned complex_data, unsigned flags);
 
+/* ---- BinaryPhaseCorrectorBlock ------------------------------------------------------------------------------------
+ * Replaces BinaryPhaseCorrectorBlock:process (radio/blocks/signal/binaryphasecorrector.lua:43-77), ComplexFloat32 in and
+ * out.  At every global sample index k*sample_interval (k = 0, 1, ..., whatever the call lengths):
+ *   phi = atan2f(im, re) folded into (-pi/2, pi/2] in double;  avg = (avg + phi/N) - last/N
+ * where N = num_samples and last is the float32 phi of measurement k-N (0 while the window fills); every sample is then
+ * multiplied by ComplexFloat32(cos(-avg), sin(-avg)) with the average after the last measurement at or before it, the
+ * product in double and rounded once.  The average and the N-entry window start at zero and are carried across calls;
+ * the measurement grid follows the consumed sample count (so seek and sharded cold starts stay on it).  Three kernel
+ * launches per call of up to 256 Mi samples.  num_samples and sample_interval must be >= 1. */
+lrb200_block_t* lrb200_phasecorrector_create(unsigned num_samples, unsigned sample_interval, unsigned flags);
+
 /* ---- IQFileSource sample formats (the source boundary, SURVEY.md 8f row 1) ------------------------------
  * Replaces the byte-swap + (value - offset) / scale loops of radio/blocks/sources/iqfile.lua:96-108 with the format
  * table of radio/utilities/format_utils.lua:82-97: u8 s8 u16le u16be s16le s16be u32le u32be s32le s32be f32le f32be

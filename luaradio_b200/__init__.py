@@ -25,7 +25,7 @@ from .signal_blocks import (MultiplyConstantBlock, UpsamplerBlock, BandpassFilte
                             HighpassFilterBlock, HilbertTransformBlock, IIRFilterBlock, LowpassFilterBlock,
                             SinglepoleHighpassFilterBlock, SinglepoleLowpassFilterBlock,
                             MultiplyBlock, MultiplyConjugateBlock, AddBlock, SubtractBlock, DelayBlock, PLLBlock, GPUMultiBlock,
-                            AGCBlock, PowerSquelchBlock)
+                            AGCBlock, PowerSquelchBlock, RootRaisedCosineFilterBlock, BinaryPhaseCorrectorBlock)
 from .types import ComplexFloat32, Float32, Vector
 from .utilities import filter_utils, spectrum_utils, window_utils
 

@@ -49,6 +49,7 @@ _PROTOS = {
     "lrb200_pll_set_mode": (c_int, [c_void_p, c_int]),
     "lrb200_agc_create": (c_void_p, [c_double, c_double, c_double, c_double, c_double, c_uint, c_uint]),
     "lrb200_powersquelch_create": (c_void_p, [c_double, c_double, c_double, c_uint, c_uint]),
+    "lrb200_phasecorrector_create": (c_void_p, [c_uint, c_uint, c_uint]),
     "lrb200_psd_create": (c_void_p, [c_uint, c_void_p, c_double, c_uint, c_uint, c_uint]),
     "lrb200_block_max_output": (c_size_t, [c_void_p, c_size_t]),
     "lrb200_block_in_size": (c_size_t, [c_void_p]),

@@ -252,6 +252,19 @@ struct LevelBlock : Block {
     long long memory_in() const override;
 };
 
+// phasecorr.cu: BinaryPhaseCorrectorBlock, a reduce / scan / apply over 2048-sample tiles (three launches per call)
+constexpr int PC_MAX_TILES = 1 << 17;      // 2048-sample tiles per launch (256 Mi samples)
+struct PhaseCorrectorBlock : Block {
+    unsigned N = 1, I = 1;                  // num_samples, sample_interval
+    DeviceBuffer d_state[2];                // {average (double), window[N] (float32, slot = measurement number mod N)}
+    int cur = 0;
+    DeviceBuffer d_tiles;                   // scratch: per-tile term sums and starting averages
+    PhaseCorrectorBlock(unsigned num_samples, unsigned sample_interval, bool dev);
+    int init() override;
+    int run(const void* dx, size_t n, void* dy, size_t* n_out, cudaStream_t s) override;
+    long long memory_in() const override;
+};
+
 }  // namespace lrb
 
 // the opaque public handle

@@ -653,6 +653,15 @@ lrb200_block_t* lrb200_powersquelch_create(double threshold_dbfs, double tau, do
     return create_block<LevelBlock>(flags, false, alpha, 0.0, 0.0, threshold, complex_data != 0);
 }
 
+// ---- digital -----------------------------------------------------------------------------------
+lrb200_block_t* lrb200_phasecorrector_create(unsigned num_samples, unsigned sample_interval, unsigned flags) {
+    if (ensure_init() != 0) return nullptr;
+    // binaryphasecorrector.lua:60 divides by num_samples and :56 pops from a num_samples-entry window
+    if (num_samples == 0) { set_error("phasecorrector: num_samples must be >= 1"); return nullptr; }
+    if (sample_interval == 0) { set_error("phasecorrector: sample_interval must be >= 1"); return nullptr; }
+    return create_block<PhaseCorrectorBlock>(flags, num_samples, sample_interval);
+}
+
 // ---- synthetic sources -------------------------------------------------------------------------
 int lrb200_synth_white_iq(complex_float32_t* dst, uint64_t n0, size_t n, uint32_t seed) {
     if (ensure_init() != 0) return -1;

@@ -525,3 +525,40 @@ class PowerSquelchBlock(GPUBlock):
         return _lib.check_handle(_lib.load().lrb200_powersquelch_create(float(self.threshold), float(self.tau), float(self.get_rate()),
                                                                         cdata, flags),
                                  "lrb200 powersquelch object")
+
+
+# ---------------------------------------------------------------------------------------------
+# Digital: the RDS / BPSK31 front ends up to clock recovery
+# ---------------------------------------------------------------------------------------------
+class RootRaisedCosineFilterBlock(FIRFilterBlock):
+    """rootraisedcosinefilter.lua:29-45: an FIR filter with root raised cosine taps (filter_utils.fir_root_raised_cosine),
+    designed in initialize() from get_rate()."""
+    name = "RootRaisedCosineFilterBlock"
+
+    def instantiate(self, num_taps, beta=None, symbol_rate=None):
+        assert num_taps is not None, "Missing argument #1 (num_taps)"
+        assert beta is not None, "Missing argument #2 (beta)"
+        assert symbol_rate is not None, "Missing argument #3 (symbol_rate)"
+        self.beta, self.symbol_rate = beta, symbol_rate
+        FIRFilterBlock.instantiate(self, Float32.vector(num_taps))
+
+    def initialize(self):
+        taps = filter_utils.fir_root_raised_cosine(self.taps.length, self.get_rate(), self.beta, 1 / self.symbol_rate)
+        self.taps = Float32.vector_from_array(taps)
+        FIRFilterBlock.initialize(self)
+
+
+class BinaryPhaseCorrectorBlock(GPUBlock):
+    """binaryphasecorrector.lua:28-77: rotates a BPSK signal against the moving average of its phase, folded into
+    (-pi/2, pi/2], measured every `sample_interval` samples over the last `num_samples` measurements."""
+    name = "BinaryPhaseCorrectorBlock"
+
+    def instantiate(self, num_samples=None, sample_interval=None):
+        assert num_samples is not None, "Missing argument #1 (num_samples)"
+        self.num_samples = num_samples
+        self.sample_interval = 32 if sample_interval is None else sample_interval
+        self.add_type_signature([Input("in", ComplexFloat32)], [Output("out", ComplexFloat32)])
+
+    def _make_handle(self, flags):
+        return _lib.check_handle(_lib.load().lrb200_phasecorrector_create(int(self.num_samples), int(self.sample_interval), flags),
+                                 "lrb200 phasecorrector object")

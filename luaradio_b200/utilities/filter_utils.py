@@ -126,3 +126,30 @@ def fir_hilbert_transform(num_taps, window_type=None):
         h.append(0.0 if n_shifted % 2 == 0 else 2.0 / (n_shifted * math.pi))
     w = window_utils.window(num_taps, window_type)
     return [a * b for a, b in zip(h, w)]
+
+
+def fir_root_raised_cosine(num_taps, sample_rate, beta, symbol_period):
+    """filter_utils.lua:301-337: root raised cosine taps, normalised to unity DC gain."""
+    if num_taps % 2 == 0:
+        raise ValueError("Number of taps must be odd.")
+
+    def approx_equal(a, b):
+        return abs(a - b) < 1e-5
+
+    h = []
+    for n in range(num_taps):
+        t = (n - (num_taps - 1) / 2) / sample_rate
+        if t == 0:
+            h.append((1 / math.sqrt(symbol_period)) * (1 - beta + 4 * beta / math.pi))
+        elif approx_equal(t, -symbol_period / (4 * beta)) or approx_equal(t, symbol_period / (4 * beta)):
+            h.append((beta / math.sqrt(2 * symbol_period)) * ((1 + 2 / math.pi) * math.sin(math.pi / (4 * beta))
+                                                             + (1 - 2 / math.pi) * math.cos(math.pi / (4 * beta))))
+        else:
+            num = (math.cos((1 + beta) * math.pi * t / symbol_period)
+                   + math.sin((1 - beta) * math.pi * t / symbol_period) / (4 * beta * t / symbol_period))
+            denom = (1 - (4 * beta * t / symbol_period) * (4 * beta * t / symbol_period))
+            h.append(((4 * beta) / (math.pi * math.sqrt(symbol_period))) * num / denom)
+    scale = 0
+    for v in h:
+        scale = scale + v
+    return [v / scale for v in h]

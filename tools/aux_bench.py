@@ -1,9 +1,10 @@
 #!/usr/bin/env python3
 """Device-side throughput of the kernels on the rows next to the hot path (SURVEY.md 8f): file sample-format converters
-at the graph boundaries, the resampling family and level control (AGCBlock, PowerSquelchBlock, the rx_am envelope chain).  One JSON object; achieved GB/s counts ALGORITHMIC bytes (input +
+at the graph boundaries, the resampling family, level control (AGCBlock, PowerSquelchBlock, the rx_am envelope chain) and
+BinaryPhaseCorrectorBlock (with the RDS signal path end to end).  One JSON object; achieved GB/s counts ALGORITHMIC bytes (input +
 output of the block), against the measured HBM peak (MEASURED_PEAKS.json, see bench.peaks()).
 
-    python tools/aux_bench.py [--samples N] [--steps K] [--only-level] > profiles/rNN_aux_bench.json
+    python tools/aux_bench.py [--samples N] [--steps K] [--only-level | --only-phasecorr] > profiles/rNN_aux_bench.json
 """
 import argparse
 import ctypes
@@ -22,6 +23,7 @@ def main():
     ap.add_argument("--steps", type=int, default=10)
     ap.add_argument("--only-resample", action="store_true", help="skip the file-format rows")
     ap.add_argument("--only-level", action="store_true", help="only the level-control rows")
+    ap.add_argument("--only-phasecorr", action="store_true", help="only the BinaryPhaseCorrectorBlock and RDS-path rows")
     args = ap.parse_args()
     import torch
     import luaradio_b200 as radio
@@ -99,6 +101,10 @@ def main():
         level_rows(lib, _lib, radio, timed, timed_calls, x, y, n)
         print(json.dumps({"peak_GBs": peak, "peak_source": src, "samples": n, "steps": args.steps, "rows": rows}))
         return
+    if args.only_phasecorr:
+        phasecorr_rows(lib, timed, timed_calls, x, y, n, rows, args.steps)
+        print(json.dumps({"card": card(), "peak_GBs": peak, "peak_source": src, "samples": n, "steps": args.steps, "rows": rows}))
+        return
 
     # ---- file formats: fill `raw` with the sink's own output so the source converters read realistic bytes
     for fmt, b in (() if args.only_resample else (("u8", 1), ("s16le", 2), ("f32be", 4))):
@@ -121,6 +127,7 @@ def main():
         timed("interpolator x%d" % L if Dn == 1 else "rational resampler %d/%d" % (L, Dn), make, x.data_ptr(), m, y.data_ptr(),
               8 + 8.0 * L / Dn, "128 taps, complex")
     level_rows(lib, _lib, radio, timed, timed_calls, x, y, n)
+    phasecorr_rows(lib, timed, timed_calls, x, y, n, rows, args.steps)
     print(json.dumps({"peak_GBs": peak, "peak_source": src, "samples": n, "steps": args.steps, "rows": rows}))
 
 
@@ -157,6 +164,68 @@ def level_rows(lib, _lib, radio, timed, timed_calls, x, y, n):
                 dev(radio.AGCBlock("slow"), Float32, af)]
     timed("rx_am envelope chain", envelope_chain, x.data_ptr(), n, y.data_ptr(), 8 + 4.0 / 25,
           "Tuner(-50e3, 10e3, 25) -> AMEnvelopeDemodulator(5e3) -> AGCBlock('slow'); bytes = chain input + output")
+
+
+def card():
+    """The card the rows ran on: name, power limit and SM clocks, read (not set) through nvidia-smi."""
+    import subprocess
+    q = "name,power.limit,clocks.max.sm,clocks.sm"
+    try:
+        out = subprocess.run(["nvidia-smi", "-i", "0", "--query-gpu=" + q, "--format=csv,noheader"], capture_output=True,
+                             text=True, timeout=30).stdout.strip()
+    except Exception as e:                       # the rows stand without it; say why it is missing
+        return {"error": str(e)}
+    return dict(zip(("name", "power_limit", "clocks_max_sm", "clocks_sm"), (v.strip() for v in out.split(","))))
+
+
+def phasecorr_rows(lib, timed, timed_calls, x, y, n, rows, steps):
+    """BinaryPhaseCorrectorBlock on white noise, 16 algorithmic bytes per sample (x read once, y written once), for
+    (N, I) = (8000, 32) (the RDS example), (50, 32) (BPSK31) and (4, 1) (a measurement every sample): one call of n samples,
+    and n / 16 samples in 8192- and 131072-sample calls.  Then the RDS signal path (examples/rtlsdr_rds.lua, TunerBlock to
+    ComplexToRealBlock) end to end through CompositeBlock.run from host memory, with the PLL serial and chunk-parallel."""
+    import time
+    import numpy as np
+    import luaradio_b200 as radio
+    from luaradio_b200 import _lib
+    D = _lib.LRB200_DEVICE
+    for N, I in ((8000, 32), (50, 32), (4, 1)):
+        label = "phasecorr(%d, %d)" % (N, I)
+        mk = lambda: lib.lrb200_phasecorrector_create(N, I, D)
+        timed(label, lambda: [mk()], x.data_ptr(), n, y.data_ptr(), 16, "one call")
+        for call in (8192, 131072):
+            timed_calls(label + ", %d-sample calls" % call, mk(), x.data_ptr(), n // 16, call, y.data_ptr(), 16,
+                        "one block, three launches per call")
+    rate, m = 1102500.0, 1 << 24
+    rng = np.random.default_rng(1)
+    t = np.arange(m) / rate
+    mpx = 0.4 * np.sin(2 * np.pi * 700 * t) + 0.1 * np.sin(2 * np.pi * 19e3 * t) + 0.05 * np.sin(2 * np.pi * 57e3 * t)
+    xs = (np.exp(1j * (2 * np.pi * 75e3 * np.cumsum(mpx) / rate + 2 * np.pi * 250e3 * t))
+          + 0.01 * (rng.standard_normal(m) + 1j * rng.standard_normal(m))).astype(np.complex64)
+    for parallel in (False, True):
+        def run():
+            src = radio.ArraySource(xs, rate, 1 << 22)
+            hil, dly = radio.HilbertTransformBlock(129), radio.DelayBlock(129)
+            pll, mix = radio.PLLBlock(1500.0, 19e3 - 100, 19e3 + 100, 3.0), radio.MultiplyConjugateBlock()
+            pll.parallel = parallel
+            rrc, bpc = radio.RootRaisedCosineFilterBlock(101, 1, 1187.5), radio.BinaryPhaseCorrectorBlock(8000)
+            top = radio.CompositeBlock()
+            top.connect(src, radio.TunerBlock(-250e3, 200e3, 5), radio.FrequencyDiscriminatorBlock(1.25), hil, dly)
+            top.connect(hil, radio.ComplexBandpassFilterBlock(129, [18e3, 20e3]), pll)
+            top.connect(dly, "out", mix, "in1")
+            top.connect(pll, "out", mix, "in2")
+            top.connect(mix, radio.LowpassFilterBlock(128, 4e3), rrc, bpc)
+            top.connect(bpc, radio.ComplexToRealBlock(), radio.ArraySink())
+            top.connect(bpc, radio.ArraySink())
+            top.connect(rrc, radio.ArraySink())
+            t0 = time.perf_counter()
+            top.run()
+            return time.perf_counter() - t0, top.describe_gpu_graph()
+        run()
+        secs = [run() for _ in range(max(1, steps // 5))]
+        s, desc = min(secs)
+        rows.append({"kernel": "rds path, PLL %s" % ("chunk-parallel" if parallel else "serial"), "graph": desc,
+                     "input_samples": m, "ms": round(s * 1e3, 2), "msamples_per_s": round(m / s / 1e6, 2),
+                     "note": "CompositeBlock.run wall time from host memory (pageable), best of %d; PLL-bound" % len(secs)})
 
 
 if __name__ == "__main__":
