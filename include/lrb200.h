@@ -27,6 +27,13 @@
  *   LRB200_DEVICE  x / y are DEVICE pointers: the call only enqueues kernels on the library
  *                  stream (lrb200_set_stream / lrb200_sync) -- graph mode, used when connected
  *                  GPU blocks share device-resident buffers (lrb200_graph_*).
+ *                  The pointers reach the kernels as given (so do dx / dy of
+ *                  lrb200_graph_execute_device).  They need only the natural alignment of their
+ *                  element: 4 bytes for float32, 8 for complex, a component's width for the raw
+ *                  file formats (a 16-byte aligned pointer may select faster kernels, never other
+ *                  results beyond float32 rounding).  A call reads no byte outside [x, x + n
+ *                  samples) and writes no byte outside [y, y + *n_out samples); the buffers may
+ *                  sit inside larger allocations next to live data (tests/test_gpu_bounds.py).
  *
  * There is NO CPU fallback anywhere in this library: without a CUDA device every create fails.
  */

@@ -34,6 +34,21 @@ def test_library_exports_every_declared_symbol():
     assert b"sm_90a" in lib.lrb200_version()
 
 
+def test_every_block_create_function_is_in_the_bounds_harness():
+    """Every lrb200_*_create entry point of the header is a case of tests/test_gpu_bounds.py (guard bands, poison,
+    unaligned placements) or is named in its commented exclusion list: a new block cannot skip the harness."""
+    from tests import test_gpu_bounds as bounds
+    hdr = open(os.path.join(ROOT, "include", "lrb200.h")).read()
+    hdr = re.sub(r"/\*.*?\*/", "", hdr, flags=re.S)
+    declared = set(re.findall(r"\b(lrb200_[a-z0-9_]*_create[a-z0-9_]*)\s*\(", hdr))
+    assert len(declared) > 20
+    covered = bounds.covered_create_functions()
+    assert not covered & bounds.BOUNDS_EXCLUDED_CREATE
+    missing = declared - covered - bounds.BOUNDS_EXCLUDED_CREATE
+    assert not missing, "create entry points without a buffer-boundary case: %s" % sorted(missing)
+    assert covered | bounds.BOUNDS_EXCLUDED_CREATE <= declared, sorted((covered | bounds.BOUNDS_EXCLUDED_CREATE) - declared)
+
+
 def test_no_cpu_fallback_without_device():
     if _have_gpu():
         pytest.skip("a GPU is present")
