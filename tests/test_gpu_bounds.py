@@ -94,15 +94,16 @@ def rnd_f(rng, n):
     return rng.uniform(-1, 1, n).astype(np.float32)
 
 
-def fir_ref(taps, x, D=1):
-    """y[n] = sum_k taps[k] x[n-k] from zero history (oracle FIRFilter), by FFT convolution in float64, every D-th."""
+def fir_ref(taps, x, D=1, wide=False):
+    """y[n] = sum_k taps[k] x[n-k] from zero history (oracle FIRFilter), by FFT convolution in float64, every D-th.
+    wide: return the float64 / complex128 result instead of rounding it to float32 / complex64."""
     import scipy.signal
-    if len(x) == 0:
-        return np.zeros(0, np.complex64 if np.iscomplexobj(x) or np.iscomplexobj(taps) else np.float32)
     cplx = np.iscomplexobj(x) or np.iscomplexobj(taps)
+    if len(x) == 0:
+        return np.zeros(0, (np.complex128 if wide else np.complex64) if cplx else (np.float64 if wide else np.float32))
     y = scipy.signal.fftconvolve(x.astype(np.complex128 if cplx else np.float64),
                                  np.asarray(taps).astype(np.complex128 if cplx else np.float64))[:len(x)][::D]
-    return y.astype(np.complex64 if cplx else np.float32)
+    return y if wide else y.astype(np.complex64 if cplx else np.float32)
 
 
 # ---- tolerance checks, each the one the block's other GPU tests use ---------------------------------------------------

@@ -333,9 +333,12 @@ def test_call_longer_than_one_launch_set():
     lib = _lib.require_device()
     n = (1 << 28) + 12345
     x = torch.empty(n, dtype=torch.complex64, device="cuda")
+    # the library stream is non-blocking: neither it nor torch's stream waits for the other, so each hand-over is a sync
     _lib.check(lib.lrb200_synth_white_iq(ctypes.c_void_p(x.data_ptr()), 0, n, 7))
+    _lib.check(lib.lrb200_sync())
     x = x + 0.8                                         # a carrier with noise: the average moves away from zero
     y1, y2 = torch.empty_like(x), torch.empty_like(x)
+    torch.cuda.synchronize()
     no = ctypes.c_size_t()
     for N, I in ((8000, 32), (17, 15)):
         one = _lib.check_handle(lib.lrb200_phasecorrector_create(N, I, _lib.LRB200_DEVICE), "phasecorr")

@@ -34,19 +34,35 @@ def _taps():
     return O.f32_taps(O.firwin_lowpass(128, 100e3 / (RATE / 2)))
 
 
-@pytest.mark.parametrize("first", [0, 1, 2, 4])
-def test_fast_fir_equals_direct_form_float64(first):
+def _shaped_taps(kind, M):
+    """Taps whose walking direction, padding and spare-tap alignment all show in the output (the low-pass is symmetric)."""
+    if kind == "random":
+        return np.random.default_rng(M).uniform(-1, 1, M).astype(np.float32)
+    h = np.zeros(M, np.float32)
+    h[{"impulse0": 0, "impulse_mid": M // 2 + 1, "impulse_last": M - 1}[kind]] = 1.0
+    return h
+
+
+FFA_CASES = [pytest.param(first, "lowpass", 128, id=str(first)) for first in (0, 1, 2, 4)] + [
+    pytest.param(first, kind, M, id="%s-m%d-first%d" % (kind, M, first))
+    for kind in ("random", "impulse0", "impulse_mid", "impulse_last") for M in (66, 67, 100, 127, 128)
+    for first in range(5)]
+
+
+@pytest.mark.parametrize("first,kind,M", FFA_CASES)
+def test_fast_fir_equals_direct_form_float64(first, kind, M):
     """Both alignment shifts (spare tap leading or trailing) and every output slot of several tiles."""
-    h = _taps()
+    h = _taps() if kind == "lowpass" else _shaped_taps(kind, M)
     tiles = 6
     xr = _rotated(tiles * K.TS * K.D + 1000)
     got, ref = K.stream(xr, h, first, tiles, exact=True)
-    assert np.max(np.abs(got - ref)) <= 1e-13
+    tol = 1e-13 if kind == "lowpass" else 1e-13 * max(1.0, float(np.sum(np.abs(h))))
+    assert np.max(np.abs(got - ref)) <= tol
     # the tiles lay out the stream's outputs y[m] = sum_k h[k] xr[first + m*D - k] (zero before the stream) in order
-    xp = np.concatenate([np.zeros(128, np.complex128), xr.astype(np.complex128)])
+    xp = np.concatenate([np.zeros(M, np.complex128), xr.astype(np.complex128)])
     m = np.arange(len(ref))
-    yref = sum(np.float64(h[k]) * xp[128 + first + m * K.D - k] for k in range(128))
-    assert np.max(np.abs(ref - yref)) <= 1e-13
+    yref = sum(np.float64(h[k]) * xp[M + first + m * K.D - k] for k in range(M))
+    assert np.max(np.abs(ref - yref)) <= tol
 
 
 def test_fast_fir_discriminator_error_float32():
