@@ -36,6 +36,10 @@
 #include "common.cuh"
 #include "blocks.h"
 
+#include <cuda.h>
+#include <cudaTypedefs.h>
+
+#include <climits>
 #include <cmath>
 #include <cstdlib>
 #include <cstring>
@@ -58,13 +62,12 @@ namespace {
 #define LRB_PT_PREFETCH 9
 #define LRB_PT_BATCH 7
 #endif
-#ifndef LRB_PT_CTAS_BULK
-// the bulk-copy interior kernel: its shared memory (44 KB per CTA) allows 5 CTAs per SM, so its register cap is set for
-// 5 rather than 8 (168 registers instead of 128: 10 warps spread over the SM's four 16 K-register partitions)
-#define LRB_PT_CTAS_BULK 5
-#endif
 #ifndef LRB_PT_EXPERIMENT
-#define LRB_PT_EXPERIMENT 0      // timing experiments only: 1 = stage the first tile only, 2 = skip the MAC loop
+// timing experiments only (wrong outputs): 1 = stage the first tile only, 2 = skip the MAC loop; of the discriminator's
+// interior kernel: 3 = no wait (after the first tile no copy is issued or waited for: later tiles compute on stale
+// shared memory), 4 = no rotation math (the tile is still copied, waited for, loaded and stored by the rotation pass),
+// 5 = no discriminator epilogue (the imaginary part of y[m] conj(y[m-1]) is stored instead of its angle)
+#define LRB_PT_EXPERIMENT 0
 #endif
 #ifndef LRB_PT_EARLY_REST
 #define LRB_PT_EARLY_REST 0
@@ -103,15 +106,16 @@ struct PolyShape {
     __host__ __device__ static constexpr int pad(int e) { return e + 2 * (e / RD); }
     static constexpr int ELEMS = LOADED + 2 * (LOADED / RD) + 2;
     static constexpr size_t SMEM = (size_t)ELEMS * sizeof(float2);
-    // bulk-copied interior tiles: the tile lands unpadded behind the padded one (RAW), and the rotation pass moves it into
-    // the padded layout, RD-sample segment by segment (stride RD + 2): each of RG thread groups takes one segment per
-    // pass, a thread one sample pair of it
-    static constexpr int RAW = ELEMS;
-    static constexpr size_t SMEM_BULK = (size_t)(ELEMS + LOADED) * sizeof(float2);
-    static constexpr int NSEG = (LOADED + RD - 1) / RD;
-    static constexpr int PPS = RD / 2;                            // sample pairs per segment
+    // tensor-copied interior tiles: one 2-D copy lands the tile straight in the padded layout, as ROWS rows of RD + 2
+    // samples read at a global row stride of RD (the rows overlap: a row's 2 pad slots receive the next row's first two
+    // samples, which the compute phase never reads there).  The rotation pass then rotates the tile in place, row by row:
+    // each of RG thread groups takes one row per pass, a thread one sample pair of it
+    static constexpr int ROWS = (SPAN + RD - 1) / RD;
+    static constexpr int STAGED = ROWS * RD + 2;                  // samples the copy reads
+    static constexpr size_t SMEM_BULK = (size_t)ROWS * (RD + 2) * sizeof(float2);
+    static constexpr int PPS = RD / 2;                            // sample pairs per row
     static constexpr int RG = PT_THREADS / PPS;
-    static constexpr int RITERS = (NSEG + RG - 1) / RG;
+    static constexpr int RITERS = (ROWS + RG - 1) / RG;
 };
 
 // ---- cp.async.bulk (global -> shared, completion counted in bytes on an mbarrier)
@@ -130,9 +134,11 @@ __device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
 }
 // orders this thread's earlier generic-proxy accesses of shared memory before its later bulk copies into it
 __device__ __forceinline__ void fence_proxy_async() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
-__device__ __forceinline__ void bulk_g2s(void* dst, const void* src, uint32_t bytes, uint64_t* bar) {
-    asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];"
-                 :: "r"(smem_addr(dst)), "l"(src), "r"(bytes), "r"(smem_addr(bar)) : "memory");
+// box {c0, c1} of a 2-D tensor map -> shared memory
+__device__ __forceinline__ void tensor_g2s_2d(void* dst, const CUtensorMap* map, int c0, int c1, uint64_t* bar) {
+    asm volatile("cp.async.bulk.tensor.2d.shared::cluster.global.tile.mbarrier::complete_tx::bytes [%0], [%1, {%2, %3}], [%4];"
+                 :: "r"(smem_addr(dst)), "l"(reinterpret_cast<uint64_t>(map)), "r"(c0), "r"(c1), "r"(smem_addr(bar))
+                 : "memory");
 }
 
 // compile-time loop: f(std::integral_constant<int, I>) for I in [B, E) -- guarantees full unrolling with
@@ -167,10 +173,10 @@ struct TileStride { static constexpr int TS = DISC ? PT_TO - DISC_OV - DISC_TAIL
 // from its predecessor beyond float32 resolution; the stream's very first run takes the carried state instead.  The
 // scan is thread-sequential (R) -> warp Kogge-Stone -> Horner over the 4 warps, both lanes at once on float2 registers.
 template <int D, int Q, bool ROT, bool DISC, bool EDGE, bool REAL = false, bool POLE = false>
-__global__ void __launch_bounds__(PT_THREADS, (!EDGE && !REAL && DISC) ? LRB_PT_CTAS_BULK : LRB_PT_CTAS)
+__global__ void __launch_bounds__(PT_THREADS, LRB_PT_CTAS)
 polyphase_crcf_kernel(const float2* __restrict__ x, const float2* __restrict__ hist, long long n,
                       void* __restrict__ yv, long long n_out, const __grid_constant__ PolyParams P,
-                      long long t_lo, long long t_hi,
+                      const __grid_constant__ CUtensorMap tmap, long long t_lo, long long t_hi,
                       const float2* __restrict__ prev_in, float2* __restrict__ prev_out, float inv_gain) {
     using S = PolyShape<D, Q>;
     static_assert(!(REAL && (ROT || DISC)), "the real-stream variant has no translator / discriminator");
@@ -182,7 +188,7 @@ polyphase_crcf_kernel(const float2* __restrict__ x, const float2* __restrict__ h
     constexpr int LANE1 = PAY * D;                                 // REAL: input distance between the two lanes' streams
     const float* __restrict__ xr = reinterpret_cast<const float*>(x);
     const float* __restrict__ histr = reinterpret_cast<const float*>(hist);
-    extern __shared__ __align__(16) float2 smem[];
+    extern __shared__ __align__(128) float2 smem[];               // (128: the tensor copy's destination)
     __shared__ float2 s_edge[PT_THREADS / 32];
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
     const int Hm1 = P.M - 1;
@@ -190,13 +196,14 @@ polyphase_crcf_kernel(const float2* __restrict__ x, const float2* __restrict__ h
     // tile-relative phasors of this thread's first sample pair, E[2 tid] and E[2 tid + 1]; the pair of staging
     // iteration `it` is 2*PT_THREADS*it samples later: E[2u] = A0 * step[it].  (A phasor TABLE in global memory
     // cost one more load stream whose latency was exposed three times per tile -- 42 % of all stall samples.)
-    // BULK: interior tiles of complex data are copied global -> shared by the copy engine (one cp.async.bulk per tile into
-    // the RAW buffer), then rotated into the padded layout.  The copy of a CTA's next tile is issued as soon as the rotation
-    // pass has read the current one, so it has the whole compute phase to land.  No staging registers and no per-thread
-    // global address arithmetic.  (One copy per padded segment instead costs a 68-iteration issue loop per tile: the copy
-    // instruction takes its operands from uniform registers.)
-    // Only the discriminator variant takes this path: it doubles the shared memory of a CTA (5 instead of 8 CTAs per SM),
-    // which made the translator-only tuner (closer to the HBM bound) 13 % slower on H100.
+    // BULK: interior tiles of complex data are copied global -> shared by the tensor-memory accelerator, one 2-D copy per
+    // tile straight into the padded layout (PolyShape::ROWS), and rotated there in place.  A CTA has one tile buffer: the
+    // copy of its next tile is issued at the epilogue's barrier, behind the compute phase's last read, and lands while the
+    // CTA finishes its epilogue and the SM's other CTAs compute.  Without a landing buffer a CTA needs 22.3 KB and 112
+    // registers, so 9 fit an SM (18 warps; the earlier landing buffer allowed 5).  No staging registers and no per-thread
+    // global address arithmetic.  (An L2 prefetch of the tile after the next one, issued with each copy, made the stage
+    // 35 % slower on H100; so did box rows RD wide with the 2 pad slots zero-filled as out-of-bounds, by 4 %.)
+    // Only the discriminator variant takes this path; the translator-only tuner keeps its register staging.
     constexpr bool BULK = !EDGE && !REAL && DISC;
     constexpr bool FFA = BULK && LRB_PT_EXPERIMENT != 2;           // fast-FIR compute phase (below)
     // FFA: per warp, lane 0's A_0 and lane 31's S, B and spare-tap sample of its last output (see the epilogue)
@@ -221,19 +228,22 @@ polyphase_crcf_kernel(const float2* __restrict__ x, const float2* __restrict__ h
         A0 = phasor_from_fix(P.turns_fix * (uint64_t)(2 * tid));
         A1 = phasor_from_fix(P.turns_fix * (uint64_t)(2 * tid + 1));
     }
-    // the last pass reaches past the tile's LOADED samples for some threads
-    const bool rot_last = rg < S::RG && (rg + S::RG * (S::RITERS - 1)) * S::RD + 2 * rw < S::LOADED;
+    // the last pass reaches past the tile's ROWS rows for some threads
+    const bool rot_last = rg < S::RG && rg + S::RG * (S::RITERS - 1) < S::ROWS;
     auto tile_of = [&](long long idx) -> long long { return EDGE ? (idx < t_lo ? idx : t_hi + (idx - t_lo)) : (t_lo + idx); };
     const long long n_work = EDGE ? 0 : (t_hi - t_lo);
     long long widx = blockIdx.x;
 
-    // thread 0 requests tile `idx` of this launch's interior range into RAW.  Callers have passed a barrier behind the
-    // last read of RAW.
+    // thread 0 requests tile `idx` of this launch's interior range into the tile buffer.  Callers have passed a barrier
+    // behind the last read of the buffer.  The tensor map's rows start at tile t_lo's first sample, and a tile starts
+    // TS * D / RD rows after its predecessor.
+    constexpr int TILE_ROWS = TS * D / S::RD;
+    static_assert(!BULK || (TS * D) % S::RD == 0, "tiles start on whole rows of the tensor map");
     auto issue_tile = [&](long long idx) {
         if (tid == 0) {
             fence_proxy_async();
-            mbar_expect_tx(&s_bar, (uint32_t)(S::LOADED * sizeof(float2)));
-            bulk_g2s(smem + S::RAW, x + (P.off + tile_of(idx) * (long long)(TS * D)), (uint32_t)(S::LOADED * sizeof(float2)), &s_bar);
+            mbar_expect_tx(&s_bar, (uint32_t)S::SMEM_BULK);
+            tensor_g2s_2d(smem, &tmap, 0, (int)(idx * TILE_ROWS), &s_bar);
         }
     };
     if constexpr (BULK) {
@@ -291,21 +301,23 @@ polyphase_crcf_kernel(const float2* __restrict__ x, const float2* __restrict__ h
         };
         if constexpr (BULK) {
             if (LRB_PT_EXPERIMENT != 1 || widx == blockIdx.x) {
-                mbar_wait(&s_bar, bar_phase);
-                bar_phase ^= 1;
+                if (LRB_PT_EXPERIMENT != 3 || widx == blockIdx.x) {
+                    mbar_wait(&s_bar, bar_phase);
+                    bar_phase ^= 1;
+                }
                 if (rg < S::RG) {
-                    const float2* src = smem + S::RAW + rg * S::RD + 2 * rw;
-                    float2* dst = smem + rg * (S::RD + 2) + 2 * rw;
+                    float2* row = smem + rg * (S::RD + 2) + 2 * rw;
 #pragma unroll
                     for (int it = 0; it < S::RITERS; ++it) {
                         if (it == S::RITERS - 1 && !rot_last) break;
-                        float4 v = *reinterpret_cast<const float4*>(src + it * S::RG * S::RD);
-                        if constexpr (ROT) {
+                        float4* p = reinterpret_cast<float4*>(row + it * S::RG * (S::RD + 2));
+                        float4 v = *p;
+                        if constexpr (ROT && LRB_PT_EXPERIMENT != 4) {
                             const float2 a = cmul(make_float2(v.x, v.y), E0[it]);
                             const float2 b = cmul(make_float2(v.z, v.w), cmul(E0[it], W1));
                             v = make_float4(a.x, a.y, b.x, b.y);
                         }
-                        *reinterpret_cast<float4*>(dst + it * S::RG * (S::RD + 2)) = v;
+                        *p = v;
                     }
                 }
             }
@@ -356,10 +368,6 @@ polyphase_crcf_kernel(const float2* __restrict__ x, const float2* __restrict__ h
         }
         __syncthreads();
 
-        // BULK: RAW has been read; the next tile's copy lands during the compute phase
-        if constexpr (BULK && LRB_PT_EXPERIMENT != 1) {
-            if (widx + gridDim.x < n_work) issue_tile(widx + gridDim.x);
-        }
         // ---- prefetch the first batch of this CTA's next tile; it stays in registers across the compute phase
         if constexpr (!EDGE && !BULK && LRB_PT_EXPERIMENT != 1) {
             const long long nidx = widx + gridDim.x;
@@ -612,6 +620,10 @@ polyphase_crcf_kernel(const float2* __restrict__ x, const float2* __restrict__ h
                 if (lane == 31) s_edge[warp] = acc[PT_R - 1];
             }
             __syncthreads();                               // also fences the shared tile for the next iteration
+            // BULK: the tile has been read; the next one is copied while this epilogue runs
+            if constexpr (BULK && LRB_PT_EXPERIMENT != 1 && LRB_PT_EXPERIMENT != 3) {
+                if (widx + gridDim.x < n_work) issue_tile(widx + gridDim.x);
+            }
             if constexpr (FFA) {
                 auto last_out = [&](int w, float2 a) {
                     return ffma2(s_ffa[3][w], make_float2(hq, hq), fsub2(fsub2(s_ffa[1][w], a), s_ffa[2][w]));
@@ -641,7 +653,8 @@ polyphase_crcf_kernel(const float2* __restrict__ x, const float2* __restrict__ h
                 // c * conj(p) = (c.x p.x + c.y p.y,  c.y p.x - c.x p.y)
                 const float2 t0 = ffma2(c0, make_float2(p0.x, p0.x), fmul2(make_float2(c0.y, -c0.x), make_float2(p0.y, p0.y)));
                 const float2 t1 = ffma2(c1, make_float2(p1.x, p1.x), fmul2(make_float2(c1.y, -c1.x), make_float2(p1.y, p1.y)));
-                const float2 ang = fast_atan2f_x2(make_float2(t0.y, t1.y), make_float2(t0.x, t1.x));
+                const float2 ang = (!EDGE && LRB_PT_EXPERIMENT == 5) ? make_float2(t0.y, t1.y)
+                                                                     : fast_atan2f_x2(make_float2(t0.y, t1.y), make_float2(t0.x, t1.x));
                 dout[r] = ang.x * inv_gain;
                 dout[r + 1] = ang.y * inv_gain;
             }
@@ -694,6 +707,37 @@ polyphase_crcf_kernel(const float2* __restrict__ x, const float2* __restrict__ h
     }
 }
 
+// the interior discriminator kernel's tensor map over x[base ..]: `rows` rows of rd + 2 samples at a row stride of rd
+// samples (consecutive rows overlap by 2 samples), a box of box_rows whole rows.  The encoder is the driver's, looked up
+// through the runtime so that the library does not link libcuda.
+int encode_tile_map(CUtensorMap* map, const float2* base, long long rows, int rd, int box_rows) {
+    static const PFN_cuTensorMapEncodeTiled encode = []() -> PFN_cuTensorMapEncodeTiled {
+        void* fn = nullptr;
+        cudaDriverEntryPointQueryResult q = cudaDriverEntryPointSymbolNotFound;
+        if (cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &fn, cudaEnableDefault, &q) != cudaSuccess ||
+            q != cudaDriverEntryPointSuccess)
+            return nullptr;
+        return reinterpret_cast<PFN_cuTensorMapEncodeTiled>(fn);
+    }();
+    if (!encode) {
+        set_error("tuner: the driver has no cuTensorMapEncodeTiled");
+        return -1;
+    }
+    // float32 elements: a sample is 2 of them
+    const cuuint64_t dims[2] = {(cuuint64_t)(2 * (rd + 2)), (cuuint64_t)rows};
+    const cuuint64_t strides[1] = {(cuuint64_t)rd * sizeof(float2)};
+    const cuuint32_t box[2] = {(cuuint32_t)(2 * (rd + 2)), (cuuint32_t)box_rows};
+    const cuuint32_t elem_strides[2] = {1, 1};
+    const CUresult r = encode(map, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 2, const_cast<float2*>(base), dims, strides, box,
+                              elem_strides, CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_NONE,
+                              CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+    if (r != CUDA_SUCCESS) {
+        set_error("tuner: cuTensorMapEncodeTiled failed (CUresult %d)", (int)r);
+        return -1;
+    }
+    return 0;
+}
+
 template <int D, int Q, bool ROT, bool DISC, bool REAL = false, bool POLE = false>
 int launch_shape(PolyParams P, const float* hr_base, const float2* x, const float2* hist, long long n,
                  void* y, long long first, long long n_out, const float2* prev_in, float2* prev_out, float inv_gain,
@@ -707,7 +751,10 @@ int launch_shape(PolyParams P, const float* hr_base, const float2* x, const floa
     int& ctas_per_sm = ctas_dev[ctx().device & (LRB_MAX_DEVICES - 1)];
     auto kern_i = polyphase_crcf_kernel<D, Q, ROT, DISC, false, REAL, POLE>;
     auto kern_e = polyphase_crcf_kernel<D, Q, ROT, DISC, true, REAL, POLE>;
-    constexpr size_t SMEM_I = (!REAL && DISC) ? S::SMEM_BULK : S::SMEM;   // interior kernel: BULK with the discriminator
+    constexpr bool BULK = !REAL && DISC;                                   // the interior kernel's tensor-copied tiles
+    constexpr size_t SMEM_I = BULK ? S::SMEM_BULK : S::SMEM;
+    static_assert(!BULK || S::SMEM_BULK >= (size_t)(S::pad(S::SPAN - 1) + 1) * sizeof(float2),
+                  "the tensor copy covers every sample a tile reads");
     if (!configured) {
         LRB_CHECK(cudaFuncSetAttribute(kern_i, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)SMEM_I));
         LRB_CHECK(cudaFuncSetAttribute(kern_e, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)S::SMEM));
@@ -732,16 +779,17 @@ int launch_shape(PolyParams P, const float* hr_base, const float2* x, const floa
     for (int q = 0; 2 * q + 1 < Q; ++q)
         for (int p = 0; p < D; ++p) P.hs[q * D + p] = P.hr[2 * q * D + p] + P.hr[(2 * q + 1) * D + p];
     const long long tiles = (n_out + TS - 1) / TS;
-    // interior tiles: every staged sample B(t) .. B(t)+LOADED-1 inside [lead, n) and x 16-byte aligned (lead > 0: the
+    // interior tiles: every staged sample B(t) .. B(t)+STAGED-1 inside [lead, n) and x 16-byte aligned (lead > 0: the
     // first samples arrive with the neighbour exchange of a sharded run, see Ctx::lead_samples)
     cudaEvent_t lead_event = ctx().lead_samples > 0 ? ctx().lead_event : nullptr;
     const long long lead = lead_event ? ctx().lead_samples : 0;
+    const long long step = (long long)TS * D;
+    constexpr int TILE_ROWS = TS * D / S::RD;
     long long t_lo = 0, t_hi = 0;
     if ((reinterpret_cast<uintptr_t>(x) & (REAL ? 7 : 15)) == 0) {
-        const long long step = (long long)TS * D;
         const long long need = lead - off;                                   // B(t) = off + t * step >= lead
         t_lo = need <= 0 ? 0 : (need + step - 1) / step;
-        const long long lim = n - (long long)S::LOADED - off - (REAL ? (long long)PAY * D : 0);
+        const long long lim = n - (long long)(BULK ? S::STAGED : S::LOADED) - off - (REAL ? (long long)PAY * D : 0);
         t_hi = lim < 0 ? 0 : lim / step + 1;
         if (t_hi > tiles) t_hi = tiles;
         if (DISC) {
@@ -750,21 +798,28 @@ int launch_shape(PolyParams P, const float* hr_base, const float2* x, const floa
             if (t_hi > tiles - 1) t_hi = tiles - 1;
         }
         if (t_lo > t_hi) t_lo = t_hi;
+        // the tensor copy's row coordinates are int32
+        if (BULK && t_hi - t_lo > (INT_MAX - S::ROWS) / TILE_ROWS) t_hi = t_lo + (INT_MAX - S::ROWS) / TILE_ROWS;
     }
     const long long n_int = t_hi - t_lo, n_edge = tiles - n_int;
+    CUtensorMap tmap;
+    std::memset(&tmap, 0, sizeof(tmap));
+    if (BULK && n_int > 0 &&
+        encode_tile_map(&tmap, x + off + t_lo * step, (n_int - 1) * TILE_ROWS + S::ROWS, S::RD, S::ROWS) != 0)
+        return -1;
     // the edge tiles (first / last few) go to the side stream so that they overlap the interior kernel
     cudaStream_t side = ((n_int > 0 && n_edge > 0) || (lead_event && n_edge > 0)) ? side_fork(s) : s;
     if (n_edge > 0) {
         if (lead_event && side != s) LRB_CHECK(cudaStreamWaitEvent(side, lead_event, 0));
         else if (lead_event) LRB_CHECK(cudaStreamWaitEvent(s, lead_event, 0));
-        kern_e<<<(unsigned)n_edge, PT_THREADS, S::SMEM, side>>>(x, hist, n, y, n_out, P, t_lo, t_hi, prev_in, prev_out, inv_gain);
+        kern_e<<<(unsigned)n_edge, PT_THREADS, S::SMEM, side>>>(x, hist, n, y, n_out, P, tmap, t_lo, t_hi, prev_in, prev_out, inv_gain);
         count_launch();
     }
     if (n_int > 0) {
         long long grid = (long long)ctx().sm_count * ctas_per_sm - ctx().reserve_ctas;
         if (grid < 1) grid = 1;
         if (grid > n_int) grid = n_int;
-        kern_i<<<(unsigned)grid, PT_THREADS, SMEM_I, s>>>(x, hist, n, y, n_out, P, t_lo, t_hi, prev_in, prev_out, inv_gain);
+        kern_i<<<(unsigned)grid, PT_THREADS, SMEM_I, s>>>(x, hist, n, y, n_out, P, tmap, t_lo, t_hi, prev_in, prev_out, inv_gain);
         count_launch();
     }
     side_join(s, side);
