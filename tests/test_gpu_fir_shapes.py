@@ -129,15 +129,18 @@ def _tuner_case(name, h, turns, gain, n0, sig, seed, calls=TUNER_CALLS, translat
     else:
         desc = ("fir_crcf[fused x2]", None)
 
+    resolved = _resolve(calls, n0, disc)
+
     def expect(x, n0):
         y = R.tuner_ref(h, x, tr, 5, n0)
         if 65 < M <= 128:
             e = R.tuner_bound(h, x, 5, n0, TUNER_T)
-        else:       # overlap-save (outside the tuner shape): its error is normwise per block
-            e = np.full(len(y), 1e-5 * max(1.0, float(np.max(np.abs(y), initial=0.0))))
+        else:       # overlap-save (outside the tuner shape): bounded per block (tests/fft_fir_ref.py)
+            from tests import fft_fir_ref
+            e = fft_fir_ref.Case("", "crcf", h, 5, tr, "auto", [(n0, resolved)]).expect(x, n0, resolved)[1]
         return (R.discrim(y, G), R.disc_bound(y, e, G), G) if disc else (y, e, None)
 
-    return Shape(name, blocks, desc, True, not disc, [(n0, _resolve(calls, n0, disc))],
+    return Shape(name, blocks, desc, True, not disc, [(n0, resolved)],
                  lambda n: signal(sig, n, seed), expect,
                  lambda x, n0: R.tuner_mutants(h, x, tr, 5, n0, G), twice=65 < M <= 128, taps=h, turns=tr, D=5)
 
@@ -354,13 +357,16 @@ class Graph:
         xb = _lib.check_handle(lib.lrb200_malloc(maxn * isz + 64), "x")
         yb = _lib.check_handle(lib.lrb200_malloc(lib.lrb200_graph_max_output(self.g, maxn) * osz + 64), "y")
         outs, pos = [], 0
+        self.launches = []             # kernels launched by each call
         try:
             for n in calls:
                 chunk = np.ascontiguousarray(x[pos:pos + n])
                 if n:
                     _lib.check(lib.lrb200_memcpy_h2d(xb + in_off, chunk.ctypes.data, n * isz), "h2d")
                 no = ctypes.c_size_t()
+                c0 = lib.lrb200_launch_count()
                 _lib.check(lib.lrb200_graph_execute_device(self.g, xb + in_off, n, yb, ctypes.byref(no)), "execute")
+                self.launches.append(lib.lrb200_launch_count() - c0)
                 host = np.empty(no.value, np.complex64 if cplx_out else np.float32)
                 if no.value:
                     _lib.check(lib.lrb200_memcpy_d2h(host.ctypes.data, yb, no.value * osz), "d2h")
