@@ -344,11 +344,7 @@ struct PllBlock : Block {
     int mode = 0;                   // 0 = exact sequential, 1 = chunk-parallel (locked loop)
     long long warm = 0;             // lead-in of the chunk-parallel form
     DeviceBuffer d_chunks;
-    PllBlock(double loop_bw_hz, double fmin_hz, double fmax_hz, double multiplier, double rate, bool dev) {
-        name = "pll";
-        in_size = 8;
-        out_size = 8;
-        dev_ptrs = dev;
+    PllBlock(double loop_bw_hz, double fmin_hz, double fmax_hz, double multiplier, double rate, bool dev) : Block("pll", 8, 8, dev) {
         num_outputs = 2;
         // pll.lua:113-131
         double bw = 2 * M_PI * (loop_bw_hz / rate);
@@ -411,21 +407,17 @@ struct PllBlock : Block {
 struct BinaryBlock : Block {
     int op;
     bool cplx;
-    std::string label;
-    BinaryBlock(int op_, bool cplx_, bool dev) : op(op_), cplx(cplx_) {
-        static const char* names[] = {"multiply", "multiplyconjugate", "add", "subtract"};
-        label = std::string(names[op]) + (cplx ? "_cc" : "_rr");
-        name = label.c_str();
-        in_size = out_size = cplx ? 8 : 4;
-        dev_ptrs = dev;
+    static constexpr const char* NAMES[] = {"multiply", "multiplyconjugate", "add", "subtract"};
+    BinaryBlock(int op_, bool cplx_, bool dev)
+        : Block(std::string(NAMES[op_]) + (cplx_ ? "_cc" : "_rr"), cplx_ ? 8 : 4, cplx_ ? 8 : 4, dev), op(op_), cplx(cplx_) {
         num_inputs = 2;
     }
     int run(const void*, size_t, void*, size_t*, cudaStream_t) override {
-        set_error("%s needs two inputs: use lrb200_block_execute_multi", name);
+        set_error("%s needs two inputs: use lrb200_block_execute_multi", name.c_str());
         return -1;
     }
     int run_multi(const void* const* dx, int nin, size_t n, void* const* dy, int nout, size_t* n_out, cudaStream_t s) override {
-        if (nin != 2 || nout != 1) { set_error("%s: expected 2 inputs and 1 output", name); return -1; }
+        if (nin != 2 || nout != 1) { set_error("%s: expected 2 inputs and 1 output", name.c_str()); return -1; }
         *n_out = n;
         if (n == 0) return 0;
         const int vec = ((reinterpret_cast<uintptr_t>(dx[0]) | reinterpret_cast<uintptr_t>(dx[1]) | reinterpret_cast<uintptr_t>(dy[0])) & 15) == 0;
@@ -451,11 +443,7 @@ struct DelayBlock : Block {
     long long D;
     DeviceBuffer d_state[2];
     int cur = 0;
-    DelayBlock(unsigned num_samples, unsigned elem, bool dev) : D(num_samples) {
-        name = "delay";
-        in_size = out_size = elem;
-        dev_ptrs = dev;
-    }
+    DelayBlock(unsigned num_samples, unsigned elem, bool dev) : Block("delay", elem, elem, dev), D(num_samples) {}
     int init() override { return carry(d_state, (size_t)D * in_size, cur); }
     long long memory_in() const override { return D; }
     int run(const void* dx, size_t n, void* dy, size_t* n_out, cudaStream_t s) override {
@@ -482,11 +470,7 @@ struct PsdBlock : Block {
     DeviceBuffer d_tw;
     DeviceBuffer d_tw1024;           // N == 1024: inter-pass twiddles of the register-resident transform
     PsdBlock(int N_, const float* window, double scale, bool log_, bool cplx_, bool dev)
-        : N(N_), cplx(cplx_), logarithmic(log_), inv_scale((float)(1.0 / scale)) {
-        name = "psd";
-        in_size = cplx ? 8 : 4;
-        out_size = 4;
-        dev_ptrs = dev;
+        : Block("psd", cplx_ ? 8 : 4, 4, dev), N(N_), cplx(cplx_), logarithmic(log_), inv_scale((float)(1.0 / scale)) {
         logN = 0;
         while ((1 << logN) < N) ++logN;
         h_window.assign(window, window + N);

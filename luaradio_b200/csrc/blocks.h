@@ -12,11 +12,12 @@
 namespace lrb {
 
 struct Block {
-    const char* name = "block";
-    size_t in_size = 8, out_size = 8;
-    bool dev_ptrs = false;
+    std::string name;
+    size_t in_size, out_size;         // element sizes in bytes
+    bool dev_ptrs;                    // run on device pointers (LRB200_DEVICE); else execute stages host vectors
     uint64_t consumed = 0;            // global index of the next input sample
 
+    Block(std::string name_, size_t in, size_t out, bool dev) : name(std::move(name_)), in_size(in), out_size(out), dev_ptrs(dev) {}
     virtual ~Block() = default;
     virtual int init() { return 0; }
     virtual size_t max_output(size_t n) const { return n; }
@@ -25,7 +26,7 @@ struct Block {
     virtual int run(const void* dx, size_t n, void* dy, size_t* n_out, cudaStream_t s) = 0;
     // blocks with several input / output ports (all inputs the same length n and element size in_size, block.lua:516-532)
     virtual int run_multi(const void* const* dx, int nin, size_t n, void* const* dy, int nout, size_t* n_out, cudaStream_t s) {
-        if (nin != 1 || nout != 1) { set_error("%s has one input and one output", name); return -1; }
+        if (nin != 1 || nout != 1) { set_error("%s has one input and one output", name.c_str()); return -1; }
         return run(dx[0], n, dy[0], n_out, s);
     }
     int execute_multi(const void* const* x, int nin, size_t n, void* const* y, int nout, size_t* n_out);
@@ -101,7 +102,6 @@ struct FirBlock : Block {
     FirFast* fast = nullptr;          // owned; deleted in fir_fft.cu, where the type is complete
     PolyTaps* poly = nullptr;
     bool gen_poly = false;            // poly_generic.cu covers this (kind, M, D)
-    std::string label;                // owns `name` when a graph rewrite renames the block
     // output-rate pole fused behind a real polyphase decimator (graph rewrite of FIR -> IIR1 -> Downsampler)
     bool has_pole = false;
     float pole_c = 0.f;
@@ -221,7 +221,6 @@ struct InterpFirBlock : Block {       // [MultiplyConstant ->] Upsampler -> FIR(
     int Tt = 0;
     bool rs_ok = false;                  // the register-tiled (L, D) polyphase kernel covers this shape (resample.cu)
     DeviceBuffer d_hist[2];
-    std::string label;
     InterpFirBlock(bool cdata, const float* taps_host, int ntaps, int interp, int decim, bool has_scale, float scale, bool dev);
     int init() override;
     size_t max_output(size_t n) const override;

@@ -63,7 +63,7 @@ static constexpr size_t HOST_CHUNK = (size_t)1 << 24;   // samples per staged ch
 int Block::execute_multi(const void* const* x, int nin, size_t n, void* const* y, int nout, size_t* n_out) {
     cudaStream_t s = ctx().stream;
     if (nin != num_inputs || nout != num_outputs) {
-        set_error("%s: expected %d input(s) and %d output(s), got %d and %d", name, num_inputs, num_outputs, nin, nout);
+        set_error("%s: expected %d input(s) and %d output(s), got %d and %d", name.c_str(), num_inputs, num_outputs, nin, nout);
         return -1;
     }
     size_t produced = 0;
@@ -129,22 +129,19 @@ int Block::reset() {
 // ---------------------------------------------------------------------------------------------
 // FIR (+ Hilbert)
 // ---------------------------------------------------------------------------------------------
-FirBlock::FirBlock(FirKind k, const void* taps_host, unsigned ntaps, unsigned decim, bool dev, bool rot, double turns_per_sample) {
+FirBlock::FirBlock(FirKind k, const void* taps_host, unsigned ntaps, unsigned decim, bool dev, bool rot, double turns_per_sample)
+    : Block(rot ? (k == FIR_CCCF ? "rot+fir_cccf" : "rot+fir_crcf")
+                : (k == FIR_CRCF ? "fir_crcf" : k == FIR_CCCF ? "fir_cccf" : k == FIR_RRRF ? "fir_rrrf" : "hilbert"),
+            (k == FIR_CRCF || k == FIR_CCCF) ? 8 : 4, k == FIR_RRRF ? 4 : 8, dev) {
     kind = k;
     M = (int)ntaps;
     D = (int)decim;
-    dev_ptrs = dev;
-    const bool cin = (k == FIR_CRCF || k == FIR_CCCF);
-    in_size = cin ? 8 : 4;
-    out_size = (cin || k == FIR_HILBERT) ? 8 : 4;
     tap_size = (k == FIR_CCCF) ? 8 : 4;
-    name = k == FIR_CRCF ? "fir_crcf" : k == FIR_CCCF ? "fir_cccf" : k == FIR_RRRF ? "fir_rrrf" : "hilbert";
     if (rot) {
         // (the fused translator forces the overlap-save path: algo is moot)
         rotate = true;
         rot_turns = turns_per_sample;
         rot_fix = turns_to_fix(turns_per_sample);
-        name = k == FIR_CCCF ? "rot+fir_cccf" : "rot+fir_crcf";
     }
     h_taps.assign((const char*)taps_host, (const char*)taps_host + (size_t)M * tap_size);
 }
@@ -203,10 +200,7 @@ int FirBlock::run(const void* dx, size_t n, void* dy, size_t* n_out, cudaStream_
 // ---------------------------------------------------------------------------------------------
 // FrequencyTranslator
 // ---------------------------------------------------------------------------------------------
-RotatorBlock::RotatorBlock(double turns_per_sample, bool dev) {
-    name = "rotator";
-    in_size = out_size = 8;
-    dev_ptrs = dev;
+RotatorBlock::RotatorBlock(double turns_per_sample, bool dev) : Block("rotator", 8, 8, dev) {
     turns = turns_per_sample;
     turns_fix = turns_to_fix(turns_per_sample);
 }
@@ -221,11 +215,7 @@ int RotatorBlock::run(const void* dx, size_t n, void* dy, size_t* n_out, cudaStr
 // ---------------------------------------------------------------------------------------------
 // FrequencyDiscriminator
 // ---------------------------------------------------------------------------------------------
-DiscrimBlock::DiscrimBlock(float gain_, bool dev) {
-    name = "discrim";
-    in_size = 8;
-    out_size = 4;
-    dev_ptrs = dev;
+DiscrimBlock::DiscrimBlock(float gain_, bool dev) : Block("discrim", 8, 4, dev) {
     gain = gain_;
 }
 int DiscrimBlock::run(const void* dx, size_t n, void* dy, size_t* n_out, cudaStream_t s) {
@@ -240,10 +230,7 @@ int DiscrimBlock::run(const void* dx, size_t n, void* dy, size_t* n_out, cudaStr
 // ---------------------------------------------------------------------------------------------
 // Downsampler
 // ---------------------------------------------------------------------------------------------
-DownsampleBlock::DownsampleBlock(unsigned factor, unsigned elem, bool dev) {
-    name = "downsample";
-    in_size = out_size = elem;
-    dev_ptrs = dev;
+DownsampleBlock::DownsampleBlock(unsigned factor, unsigned elem, bool dev) : Block("downsample", elem, elem, dev) {
     D = (int)factor;
 }
 size_t DownsampleBlock::max_output(size_t n) const { return D == 1 ? n : n / D + 1; }
@@ -259,10 +246,8 @@ int DownsampleBlock::run(const void* dx, size_t n, void* dy, size_t* n_out, cuda
 // ---------------------------------------------------------------------------------------------
 // IIR (single pole: na <= 2)
 // ---------------------------------------------------------------------------------------------
-IirBlock::IirBlock(bool cplx, const float* b_, unsigned nb_, const float* a_, unsigned na_, bool dev) {
-    name = cplx ? "iir_crcf" : "iir_rrrf";
-    in_size = out_size = cplx ? 8 : 4;
-    dev_ptrs = dev;
+IirBlock::IirBlock(bool cplx, const float* b_, unsigned nb_, const float* a_, unsigned na_, bool dev)
+    : Block(cplx ? "iir_crcf" : "iir_rrrf", cplx ? 8 : 4, cplx ? 8 : 4, dev) {
     complex_data = cplx;
     nb = (int)nb_;
     double a0 = a_[0];
@@ -298,10 +283,8 @@ int IirBlock::run(const void* dx, size_t n, void* dy, size_t* n_out, cudaStream_
 // ---------------------------------------------------------------------------------------------
 // IIR of any order
 // ---------------------------------------------------------------------------------------------
-IirGeneralBlock::IirGeneralBlock(bool cplx, const float* b_, unsigned nb_, const float* a_, unsigned na_, bool dev) {
-    name = cplx ? "iir_crcf(general)" : "iir_rrrf(general)";
-    in_size = out_size = cplx ? 8 : 4;
-    dev_ptrs = dev;
+IirGeneralBlock::IirGeneralBlock(bool cplx, const float* b_, unsigned nb_, const float* a_, unsigned na_, bool dev)
+    : Block(cplx ? "iir_crcf(general)" : "iir_rrrf(general)", cplx ? 8 : 4, cplx ? 8 : 4, dev) {
     complex_data = cplx;
     nb = (int)nb_;
     na = (int)na_;
@@ -341,13 +324,7 @@ int IirGeneralBlock::run(const void* dx, size_t n, void* dy, size_t* n_out, cuda
 // ---------------------------------------------------------------------------------------------
 // ComplexMagnitude / ComplexToReal
 // ---------------------------------------------------------------------------------------------
-C2fBlock::C2fBlock(int op_, bool dev) {
-    op = op_;
-    name = op == 0 ? "cmag" : "c2r";
-    in_size = 8;
-    out_size = 4;
-    dev_ptrs = dev;
-}
+C2fBlock::C2fBlock(int op_, bool dev) : Block(op_ == 0 ? "cmag" : "c2r", 8, 4, dev) { op = op_; }
 int C2fBlock::run(const void* dx, size_t n, void* dy, size_t* n_out, cudaStream_t s) {
     *n_out = n;
     consumed += n;
@@ -496,15 +473,15 @@ int lrb200_memset(void* p, int value, size_t bytes) {
 // ---- generic block ---------------------------------------------------------------------------
 int lrb200_block_execute(lrb200_block_t* q, const void* x, size_t n, void* y, size_t* n_out) {
     if (!q || !q->impl) { set_error("null block handle"); return -1; }
-    if (n > 0 && (!x || !y)) { set_error("%s: null sample buffer", q->impl->name); return -1; }
+    if (n > 0 && (!x || !y)) { set_error("%s: null sample buffer", q->impl->name.c_str()); return -1; }
     return q->impl->execute(x, n, y, n_out);
 }
 int lrb200_block_execute_multi(lrb200_block_t* q, const void* const* x, unsigned num_inputs, size_t n, void* const* y,
                                unsigned num_outputs, size_t* n_out) {
     if (!q || !q->impl) { set_error("null block handle"); return -1; }
-    if (!x || !y) { set_error("%s: null port array", q->impl->name); return -1; }
-    for (unsigned i = 0; i < num_inputs; ++i) if (n > 0 && !x[i]) { set_error("%s: null sample buffer", q->impl->name); return -1; }
-    for (unsigned i = 0; i < num_outputs; ++i) if (n > 0 && !y[i]) { set_error("%s: null sample buffer", q->impl->name); return -1; }
+    if (!x || !y) { set_error("%s: null port array", q->impl->name.c_str()); return -1; }
+    for (unsigned i = 0; i < num_inputs; ++i) if (n > 0 && !x[i]) { set_error("%s: null sample buffer", q->impl->name.c_str()); return -1; }
+    for (unsigned i = 0; i < num_outputs; ++i) if (n > 0 && !y[i]) { set_error("%s: null sample buffer", q->impl->name.c_str()); return -1; }
     return q->impl->execute_multi(x, (int)num_inputs, n, y, (int)num_outputs, n_out);
 }
 unsigned lrb200_block_num_inputs(const lrb200_block_t* q) { return q && q->impl ? (unsigned)q->impl->num_inputs : 0; }
@@ -525,7 +502,7 @@ void lrb200_block_destroy(lrb200_block_t* q) {
     delete q->impl;
     delete q;
 }
-const char* lrb200_block_name(const lrb200_block_t* q) { return q && q->impl ? q->impl->name : ""; }
+const char* lrb200_block_name(const lrb200_block_t* q) { return q && q->impl ? q->impl->name.c_str() : ""; }
 
 // ---- FIR ---------------------------------------------------------------------------------------
 static lrb200_block_t* fir_create(FirKind k, const void* taps, unsigned ntaps, unsigned decim, unsigned flags) {

@@ -17,8 +17,9 @@ struct Ctx {
     cudaStream_t stream = nullptr;
     bool own_stream = false;
     std::atomic<uint64_t> launches{0};
-    // persistent kernels leave this many CTA slots free while a sharded run has a head piece queued on another stream
-    // (graph.cu: run_shard) -- otherwise the head's few small kernels only get an SM once the persistent grid drains
+    // persistent kernels leave this many CTA slots free while the first stage of a sharded run keeps its edge tiles waiting
+    // for the neighbour's halo on the side stream (graph.cu: run_shard) -- otherwise those few tiles only get an SM once
+    // the persistent grid drains
     int reserve_ctas = 0;
     // time-chunk sharding: the first `lead_samples` input samples of the launch in flight come from the left neighbour and
     // are only valid after `lead_event`; the polyphase launcher keeps every tile that touches them out of the interior

@@ -4,11 +4,7 @@
 // pipes (radio/core/composite.lua:568-636, radio/core/pipe.lua:53-88): intermediate sample vectors stay
 // in a two-slot device ring; host<->device traffic exists only at the two ends, double-buffered on
 // separate copy streams so chunk i+1 uploads while chunk i computes and chunk i-1 downloads.
-// commit(fuse=1) rewrites adjacent blocks into fused kernels:
-//   Rotator -> FIR(crcf) -> Downsampler [-> Discriminator]  =>  tuner kernel (composites/tuner.lua:40-47)
-//   FIR -> Downsampler                    =>  decimating FIR    (composites/decimator.lua:34-41)
-//   IIR -> Downsampler                    =>  scan with strided store
-//   [MultiplyConstant ->] Upsampler -> FIR [-> Downsampler]  =>  polyphase interpolating FIR
+// commit(fuse=1) rewrites runs of adjacent blocks into fused kernels, one rule function per rewrite (below).
 #include "../../include/lrb200.h"
 #include "common.cuh"
 #include "blocks.h"
@@ -23,9 +19,156 @@
 
 namespace lrb {
 
-struct Graph {
-    std::vector<std::unique_ptr<Block>> blocks;   // as appended
-    std::vector<std::unique_ptr<Block>> fused;    // blocks created by fusion
+using Blocks = std::vector<std::unique_ptr<Block>>;
+
+// What a rule made of the run starting at blocks[i]: one stage, or two, standing for the first `used` blocks.
+struct Rewrite {
+    std::unique_ptr<Block> stage, stage2;
+    size_t used = 0;                 // 0: no match
+};
+// 0 (a match or none, see out->used), or -1 with the error set
+using Rule = int (*)(const Blocks& blocks, size_t i, Rewrite* out);
+
+// blocks[j] as a T, or nullptr (another type, or past the end)
+template <class T> T* block_at(const Blocks& blocks, size_t j) {
+    return j < blocks.size() ? dynamic_cast<T*>(blocks[j].get()) : nullptr;
+}
+
+// Rotator -> FIR(crcf, D = 1) -> Downsampler(8 B) [-> Discriminator]  =>  tuner kernel (composites/tuner.lua:40-47).
+// No match when the tuner kernel has no instantiation for the (taps, decimation) shape.
+static int fuse_tuner(const Blocks& blocks, size_t i, Rewrite* out) {
+    RotatorBlock* rot = block_at<RotatorBlock>(blocks, i);
+    FirBlock* fir = block_at<FirBlock>(blocks, i + 1);
+    DownsampleBlock* down = block_at<DownsampleBlock>(blocks, i + 2);
+    if (!rot || !fir || fir->kind != FIR_CRCF || fir->D != 1 || !down || down->in_size != 8) return 0;
+    DiscrimBlock* disc = block_at<DiscrimBlock>(blocks, i + 3);
+    out->stage = make_tuner(rot->turns, (const float*)fir->h_taps.data(), fir->M, down->D, disc ? disc->gain : 0.0f);
+    if (out->stage) out->used = disc ? 4 : 3;
+    return 0;
+}
+
+// Rotator -> FIR(crcf or cccf, D = 1, M <= 513) [-> Downsampler(8 B)]  =>  overlap-save FIR with the translator folded in
+// (any taps, complex taps included)
+static int fuse_rotator_overlap_save(const Blocks& blocks, size_t i, Rewrite* out) {
+    RotatorBlock* rot = block_at<RotatorBlock>(blocks, i);
+    FirBlock* fir = block_at<FirBlock>(blocks, i + 1);
+    if (!rot || !fir || (fir->kind != FIR_CRCF && fir->kind != FIR_CCCF) || fir->D != 1 || fir->M > 513) return 0;
+    DownsampleBlock* down = block_at<DownsampleBlock>(blocks, i + 2);
+    if (down && down->in_size != 8) down = nullptr;
+    out->stage = make_block<FirBlock>(fir->kind, fir->h_taps.data(), (unsigned)fir->M, (unsigned)(down ? down->D : 1), true, true,
+                                      rot->turns);
+    if (!out->stage) return -1;
+    out->used = down ? 3 : 2;
+    return 0;
+}
+
+// [MultiplyConstant(real c) ->] Upsampler(L) -> FIR(crcf or rrrf, D = 1) [-> Downsampler(D)]  =>  polyphase interpolating
+// FIR (composites/interpolator.lua:31-41, composites/rationalresampler.lua:33-46).  A complex constant is not absorbed.
+static int fuse_interpolator(const Blocks& blocks, size_t i, Rewrite* out) {
+    ScaleBlock* sc = block_at<ScaleBlock>(blocks, i);
+    if (sc && sc->complex_const) sc = nullptr;
+    const size_t j = sc ? i + 1 : i;
+    UpsampleBlock* up = block_at<UpsampleBlock>(blocks, j);
+    FirBlock* fir = block_at<FirBlock>(blocks, j + 1);
+    if (!up || !fir || fir->D != 1 || (fir->kind != FIR_CRCF && fir->kind != FIR_RRRF) || fir->in_size != up->out_size) return 0;
+    DownsampleBlock* down = block_at<DownsampleBlock>(blocks, j + 2);
+    if (down && down->in_size != fir->out_size) down = nullptr;
+    out->stage = make_block<InterpFirBlock>(fir->kind == FIR_CRCF, (const float*)fir->h_taps.data(), fir->M, up->L,
+                                            down ? down->D : 1, sc != nullptr, sc ? sc->cre : 1.0f, true);
+    if (!out->stage) return -1;
+    out->used = (j - i) + 2 + (down ? 1 : 0);
+    return 0;
+}
+
+// FIR(h, rrrf, D = 1) -> single-pole IIR(b, c, real) -> Downsampler(D > 1): the chain's audio tail
+// (examples/rtlsdr_wbfm_mono.lua:15-18; iirfilter.lua:147-179; downsampler.lua:45-53).
+// y[n] = c y[n-1] + v[n], v = b * u, u = h * x.  Unrolling the recurrence D times:
+//     y[n] = c^D y[n-D] + sum_{i<D} c^i v[n-i]
+// so the kept samples z[m] = y[mD] obey  z[m] = c^D z[m-1] + w[mD]  with  w = (h * b * [1, c, .., c^(D-1)]) * x:
+// ONE decimating FIR with M + nb + D - 2 taps (only kept outputs computed) and a pole c^D at the
+// output rate, instead of a full-rate FIR and a full-rate recurrence that both compute D times more
+// samples than the Downsampler keeps.  Zero initial state on both sides, so the streams are equal
+// from the first sample; the taps are designed in float64 from the float32 coefficients.
+// One stage with the pole fused in when its memory fits the polyphase kernel's warm-up, else two stages
+// `fir*iir1_rrrf(..) | pole_rrrf`; no match when the polyphase kernel has no shape for the composed taps.
+static int fuse_noble_identity(const Blocks& blocks, size_t i, Rewrite* out) {
+    FirBlock* fir = block_at<FirBlock>(blocks, i);
+    IirBlock* iir = block_at<IirBlock>(blocks, i + 1);
+    DownsampleBlock* down = block_at<DownsampleBlock>(blocks, i + 2);
+    if (!fir || fir->D != 1 || fir->kind != FIR_RRRF || !iir || iir->complex_data || iir->D != 1 || !down || down->in_size != 4 ||
+        down->D <= 1)
+        return 0;
+    const int Dd = down->D, nbb = iir->nb;
+    std::vector<double> g((size_t)(nbb + Dd - 1), 0.0);
+    double cp = 1.0;
+    for (int k = 0; k < Dd; ++k) {
+        for (int j = 0; j < nbb; ++j) g[(size_t)(k + j)] += cp * (double)iir->b[j];
+        cp *= (double)iir->c;
+    }
+    const float* h = (const float*)fir->h_taps.data();
+    const int Mc = fir->M + (int)g.size() - 1;
+    std::vector<float> hc((size_t)Mc);
+    for (int t = 0; t < Mc; ++t) {
+        double acc = 0.0;
+        for (int k = 0; k < (int)g.size(); ++k)
+            if (t - k >= 0 && t - k < fir->M) acc += g[(size_t)k] * (double)h[t - k];
+        hc[(size_t)t] = (float)acc;
+    }
+    auto nf = make_block<FirBlock>(FIR_RRRF, hc.data(), (unsigned)Mc, (unsigned)Dd, true);
+    if (!nf) return -1;
+    nf->set_algorithm(fir->algo);
+    if (!nf->poly) return 0;         // only worth it when the polyphase kernel has this shape
+    nf->name = "fir*iir1_rrrf(" + std::to_string(Mc) + ",/" + std::to_string(Dd) + ")";
+    if (nf->algo != LRB200_FIR_FFT && polyphase_pole_ok((float)cp)) {
+        // the pole's memory (|c^D|^64 <= 1e-8) fits the kernel's own warm-up: ONE stage
+        if (nf->set_pole((float)cp) != 0) return -1;
+        nf->name += "+pole";
+    } else {
+        const float one = 1.0f, a2[2] = {1.0f, (float)(-cp)};     // cp == c^D
+        out->stage2 = make_block<IirBlock>(false, &one, 1u, a2, 2u, true);
+        if (!out->stage2) return -1;
+        out->stage2->name = "pole_rrrf";
+    }
+    out->stage = std::move(nf);
+    out->used = 3;
+    return 0;
+}
+
+// FIR(D = 1, not Hilbert) -> Downsampler(D)  =>  decimating FIR (composites/decimator.lua:34-41)
+static int fuse_fir_decimator(const Blocks& blocks, size_t i, Rewrite* out) {
+    FirBlock* fir = block_at<FirBlock>(blocks, i);
+    DownsampleBlock* down = block_at<DownsampleBlock>(blocks, i + 1);
+    if (!fir || fir->D != 1 || fir->kind == FIR_HILBERT || !down || down->in_size != fir->out_size) return 0;
+    auto nf = make_block<FirBlock>(fir->kind, fir->h_taps.data(), (unsigned)fir->M, (unsigned)down->D, true);
+    if (!nf) return -1;
+    nf->set_algorithm(fir->algo);    // FIRFilterBlock(taps, use_fft) survives the fusion
+    out->stage = std::move(nf);
+    out->used = 2;
+    return 0;
+}
+
+// single-pole IIR(D = 1) -> Downsampler(D)  =>  scan with strided store
+static int fuse_iir_decimator(const Blocks& blocks, size_t i, Rewrite* out) {
+    IirBlock* iir = block_at<IirBlock>(blocks, i);
+    DownsampleBlock* down = block_at<DownsampleBlock>(blocks, i + 1);
+    if (!iir || iir->D != 1 || !down || down->in_size != iir->out_size) return 0;
+    const float a[2] = {1.0f, -iir->c};
+    auto ni = make_block<IirBlock>(iir->complex_data, iir->b, (unsigned)iir->nb, a, 2u, true);
+    if (!ni) return -1;
+    ni->D = down->D;
+    out->stage = std::move(ni);
+    out->used = 2;
+    return 0;
+}
+
+// in priority order: the first rule that matches at a block wins
+static const Rule FUSION_RULES[] = {fuse_tuner, fuse_rotator_overlap_save, fuse_interpolator, fuse_noble_identity,
+                                   fuse_fir_decimator, fuse_iir_decimator};
+
+// A committed linear run of blocks, itself a one-port Block (a node of a Dag).  Its name is the description.
+struct Graph : Block {
+    Blocks blocks;                   // as appended
+    Blocks fused;                    // blocks created by fusion
     std::vector<Block*> stages;      // execution order after commit (not owned)
     bool committed = false;
     DeviceBuffer ring[2];
@@ -34,7 +177,6 @@ struct Graph {
     cudaStream_t s_h2d = nullptr, s_d2h = nullptr;
     cudaEvent_t ev_h2d[2] = {nullptr, nullptr}, ev_comp[2] = {nullptr, nullptr}, ev_d2h[2] = {nullptr, nullptr};
     size_t host_chunk = (size_t)1 << 23;   // input samples per pipelined chunk
-    std::string desc;
     // super-chunk mode (SURVEY.md 8e "streaming mode"): small host vectors are packed into pinned slots of `sc` samples;
     // a full slot is processed asynchronously while the next one fills, and its outputs are handed back when that next
     // slot is submitted (or at flush) -- the per-vector cost is one host memcpy instead of copies + launches + a sync
@@ -55,14 +197,26 @@ struct Graph {
     std::vector<std::vector<cudaEvent_t>> tev;   // per stage: [start0, stop0, start1, stop1, ...]
     std::vector<int> tcount;
 
+    Graph() : Block("", 8, 8, true) {}      // element sizes and name (the description) are set by commit
+
     cudaEvent_t timing_event(size_t stage, size_t idx) {
-        if (tev.size() < stages.size()) { tev.resize(stages.size()); tcount.assign(stages.size(), 0); }
         auto& v = tev[stage];
         while (v.size() <= idx) { cudaEvent_t e; cudaEventCreate(&e); v.push_back(e); }
         return v[idx];
     }
+    // per-stage timing: events recorded on s around stage k's launches
+    void timing_start(size_t k, cudaStream_t s) {
+        if (!timing) return;
+        if (tcount.size() < stages.size()) { tev.resize(stages.size()); tcount.assign(stages.size(), 0); }
+        cudaEventRecord(timing_event(k, 2 * (size_t)tcount[k]), s);
+    }
+    void timing_stop(size_t k, cudaStream_t s) {
+        if (!timing) return;
+        cudaEventRecord(timing_event(k, 2 * (size_t)tcount[k] + 1), s);
+        tcount[k]++;
+    }
 
-    ~Graph() {
+    ~Graph() override {
         for (auto& v : tev) for (cudaEvent_t e : v) cudaEventDestroy(e);
         for (int i = 0; i < 2; ++i) {
             if (ev_h2d[i]) cudaEventDestroy(ev_h2d[i]);
@@ -85,176 +239,84 @@ struct Graph {
         sc = 0; sc_fill = 0; sc_cur = 0;
     }
 
-    size_t max_output(size_t n) const {
+    size_t max_output(size_t n) const override {
         for (Block* b : stages) n = b->max_output(n);
         return n;
+    }
+    uint64_t outputs_before(uint64_t idx) const override {
+        for (Block* b : stages) idx = b->outputs_before(idx);
+        return idx;
+    }
+    void rate(unsigned* up, unsigned* down) const override {
+        unsigned long long u, d;
+        total_rate(&u, &d);
+        *up = (unsigned)u; *down = (unsigned)d;
     }
 
     int commit(int fuse) {
         stages.clear();
         fused.clear();
-        desc.clear();
-        size_t i = 0;
-        while (i < blocks.size()) {
-            Block* b = blocks[i].get();
-            Block* st = b;
-            Block* st2 = nullptr;        // a rewrite may turn a run of blocks into two stages
-            size_t used = 1;
-            if (fuse) {
-                RotatorBlock* rot = dynamic_cast<RotatorBlock*>(b);
-                FirBlock* fir = dynamic_cast<FirBlock*>(b);
-                IirBlock* iir = dynamic_cast<IirBlock*>(b);
-                if (rot && i + 1 < blocks.size()) {
-                    FirBlock* f2 = dynamic_cast<FirBlock*>(blocks[i + 1].get());
-                    DownsampleBlock* d3 = (i + 2 < blocks.size()) ? dynamic_cast<DownsampleBlock*>(blocks[i + 2].get()) : nullptr;
-                    if (d3 && d3->in_size != 8) d3 = nullptr;
-                    const bool fir_ok = f2 && (f2->kind == FIR_CRCF || f2->kind == FIR_CCCF) && f2->D == 1;
-                    if (fir_ok && d3 && f2->kind == FIR_CRCF) {
-                        DiscrimBlock* d4 = (i + 3 < blocks.size()) ? dynamic_cast<DiscrimBlock*>(blocks[i + 3].get()) : nullptr;
-                        std::unique_ptr<Block> t = make_tuner(rot->turns, (const float*)f2->h_taps.data(), f2->M, d3->D, d4 ? d4->gain : 0.0f);
-                        if (t) { st = t.get(); fused.push_back(std::move(t)); used = d4 ? 4 : 3; }
-                    }
-                    if (used == 1 && fir_ok && f2->M <= 513) {
-                        // translator folded into the overlap-save kernel (any taps, complex taps included)
-                        auto nf = make_block<FirBlock>(f2->kind, f2->h_taps.data(), (unsigned)f2->M, (unsigned)(d3 ? d3->D : 1), true,
-                                                       true, rot->turns);
-                        if (!nf) return -1;
-                        st = nf.get(); fused.push_back(std::move(nf)); used = d3 ? 3 : 2;
-                    }
+        name.clear();
+        for (size_t i = 0; i < blocks.size();) {
+            Rewrite rw;
+            if (fuse)
+                for (Rule rule : FUSION_RULES) {
+                    if (rule(blocks, i, &rw) != 0) return -1;
+                    if (rw.used) break;
                 }
-                {
-                    // [MultiplyConstant(real c) ->] Upsampler(L) -> FIR(real taps) [-> Downsampler(D)]  =>  polyphase
-                    // interpolating FIR (composites/interpolator.lua:31-41, composites/rationalresampler.lua:33-46)
-                    size_t j = i;
-                    ScaleBlock* sc = dynamic_cast<ScaleBlock*>(blocks[j].get());
-                    if (sc && !sc->complex_const) ++j; else sc = nullptr;
-                    UpsampleBlock* up = j < blocks.size() ? dynamic_cast<UpsampleBlock*>(blocks[j].get()) : nullptr;
-                    FirBlock* f2 = (up && j + 1 < blocks.size()) ? dynamic_cast<FirBlock*>(blocks[j + 1].get()) : nullptr;
-                    if (up && f2 && f2->D == 1 && (f2->kind == FIR_CRCF || f2->kind == FIR_RRRF) && f2->in_size == up->out_size) {
-                        DownsampleBlock* d3 = (j + 2 < blocks.size()) ? dynamic_cast<DownsampleBlock*>(blocks[j + 2].get()) : nullptr;
-                        if (d3 && d3->in_size != f2->out_size) d3 = nullptr;
-                        auto nb = make_block<InterpFirBlock>(f2->kind == FIR_CRCF, (const float*)f2->h_taps.data(), f2->M, up->L,
-                                                             d3 ? d3->D : 1, sc != nullptr, sc ? sc->cre : 1.0f, true);
-                        if (!nb) return -1;
-                        st = nb.get(); fused.push_back(std::move(nb)); used = (j - i) + 2 + (d3 ? 1 : 0);
-                    }
-                }
-                if (used == 1 && fir && fir->D == 1 && fir->kind == FIR_RRRF && i + 2 < blocks.size()) {
-                    // FIR(h) -> single-pole IIR (b, c) -> Downsampler(D), all real (the chain's audio tail,
-                    // examples/rtlsdr_wbfm_mono.lua:15-18; iirfilter.lua:147-179; downsampler.lua:45-53).
-                    // y[n] = c y[n-1] + v[n], v = b * u, u = h * x.  Unrolling the recurrence D times:
-                    //     y[n] = c^D y[n-D] + sum_{i<D} c^i v[n-i]
-                    // so the kept samples z[m] = y[mD] obey  z[m] = c^D z[m-1] + w[mD]  with  w = (h * b * [1, c, .., c^(D-1)]) * x:
-                    // ONE decimating FIR with M + nb + D - 2 taps (only kept outputs computed) and a pole c^D at the
-                    // output rate, instead of a full-rate FIR and a full-rate recurrence that both compute D times more
-                    // samples than the Downsampler keeps.  Zero initial state on both sides, so the streams are equal
-                    // from the first sample; the taps are designed in float64 from the float32 coefficients.
-                    IirBlock* i2 = dynamic_cast<IirBlock*>(blocks[i + 1].get());
-                    DownsampleBlock* d3 = dynamic_cast<DownsampleBlock*>(blocks[i + 2].get());
-                    if (i2 && !i2->complex_data && i2->D == 1 && d3 && d3->in_size == 4 && d3->D > 1) {
-                        const int Dd = d3->D, nbb = i2->nb;
-                        std::vector<double> g((size_t)(nbb + Dd - 1), 0.0);
-                        double cp = 1.0;
-                        for (int k = 0; k < Dd; ++k) {
-                            for (int j = 0; j < nbb; ++j) g[(size_t)(k + j)] += cp * (double)i2->b[j];
-                            cp *= (double)i2->c;
-                        }
-                        const float* h = (const float*)fir->h_taps.data();
-                        const int Mc = fir->M + (int)g.size() - 1;
-                        std::vector<float> hc((size_t)Mc);
-                        for (int t = 0; t < Mc; ++t) {
-                            double acc = 0.0;
-                            for (int k = 0; k < (int)g.size(); ++k)
-                                if (t - k >= 0 && t - k < fir->M) acc += g[(size_t)k] * (double)h[t - k];
-                            hc[(size_t)t] = (float)acc;
-                        }
-                        auto nf = make_block<FirBlock>(FIR_RRRF, hc.data(), (unsigned)Mc, (unsigned)Dd, true);
-                        if (!nf) return -1;
-                        nf->set_algorithm(fir->algo);
-                        if (nf->poly && nf->algo != LRB200_FIR_FFT && polyphase_pole_ok((float)cp)) {
-                            // the pole's memory (|c^D|^64 <= 1e-8) fits the kernel's own warm-up: ONE stage
-                            if (nf->set_pole((float)cp) != 0) return -1;
-                            nf->label = "fir*iir1_rrrf(" + std::to_string(Mc) + ",/" + std::to_string(Dd) + ")+pole";
-                            nf->name = nf->label.c_str();
-                            st = nf.get(); used = 3;
-                            fused.push_back(std::move(nf));
-                        } else if (nf->poly) {      // only worth it when the polyphase kernel has this shape
-                            const float one = 1.0f, a2[2] = {1.0f, (float)(-cp)};     // cp == c^D
-                            auto ni = make_block<IirBlock>(false, &one, 1u, a2, 2u, true);
-                            if (!ni) return -1;
-                            nf->label = "fir*iir1_rrrf(" + std::to_string(Mc) + ",/" + std::to_string(Dd) + ")";
-                            nf->name = nf->label.c_str();
-                            ni->name = "pole_rrrf";
-                            st = nf.get(); st2 = ni.get(); used = 3;
-                            fused.push_back(std::move(nf)); fused.push_back(std::move(ni));
-                        }
-                    }
-                }
-                if (used == 1 && fir && fir->D == 1 && fir->kind != FIR_HILBERT && i + 1 < blocks.size()) {
-                    DownsampleBlock* d2 = dynamic_cast<DownsampleBlock*>(blocks[i + 1].get());
-                    if (d2 && d2->in_size == fir->out_size) {
-                        auto nf = make_block<FirBlock>(fir->kind, fir->h_taps.data(), (unsigned)fir->M, (unsigned)d2->D, true);
-                        if (!nf) return -1;
-                        nf->set_algorithm(fir->algo);      // FIRFilterBlock(taps, use_fft) survives the fusion
-                        st = nf.get(); fused.push_back(std::move(nf)); used = 2;
-                    }
-                }
-                if (used == 1 && iir && iir->D == 1 && i + 1 < blocks.size()) {
-                    DownsampleBlock* d2 = dynamic_cast<DownsampleBlock*>(blocks[i + 1].get());
-                    if (d2 && d2->in_size == iir->out_size) {
-                        float a[2] = {1.0f, -iir->c};
-                        auto ni = make_block<IirBlock>(iir->complex_data, iir->b, (unsigned)iir->nb, a, 2u, true);
-                        if (!ni) return -1;
-                        ni->D = d2->D;
-                        st = ni.get(); fused.push_back(std::move(ni)); used = 2;
-                    }
-                }
-            }
+            Block* st = blocks[i].get();
+            if (rw.used) { st = rw.stage.get(); fused.push_back(std::move(rw.stage)); }
             stages.push_back(st);
-            if (!desc.empty()) desc += " | ";
-            desc += st->name;
-            if (used > 1) { desc += "[fused x"; desc += std::to_string(used); desc += "]"; }
-            if (st2) { stages.push_back(st2); desc += " | "; desc += st2->name; }
-            i += used;
+            if (!name.empty()) name += " | ";
+            name += st->name;
+            if (rw.used > 1) name += "[fused x" + std::to_string(rw.used) + "]";
+            if (rw.stage2) {
+                stages.push_back(rw.stage2.get());
+                name += " | " + rw.stage2->name;
+                fused.push_back(std::move(rw.stage2));
+            }
+            i += rw.used ? rw.used : 1;
         }
         for (size_t k = 0; k + 1 < stages.size(); ++k) {
             if (stages[k]->out_size != stages[k + 1]->in_size) {
-                set_error("graph: %s (out %zu B) cannot feed %s (in %zu B)", stages[k]->name, stages[k]->out_size,
-                          stages[k + 1]->name, stages[k + 1]->in_size);
+                set_error("graph: %s (out %zu B) cannot feed %s (in %zu B)", stages[k]->name.c_str(), stages[k]->out_size,
+                          stages[k + 1]->name.c_str(), stages[k + 1]->in_size);
                 return -1;
             }
         }
+        if (!stages.empty()) { in_size = stages.front()->in_size; out_size = stages.back()->out_size; }
         committed = true;
+        return 0;
+    }
+    int ensure_committed() { return committed ? 0 : commit(1); }
+
+    // grow the two-slot ring for a call of n inputs; a stage still in flight may be reading the old buffer
+    int reserve_ring(size_t n, cudaStream_t s) {
+        for (size_t k = 0; k + 1 < stages.size(); ++k) {
+            n = stages[k]->max_output(n);
+            const size_t bytes = (n ? n : 1) * stages[k]->out_size;
+            DeviceBuffer& slot = ring[k & 1];
+            if (bytes > slot.capacity()) {
+                LRB_CHECK(cudaStreamSynchronize(s));
+                if (slot.reserve(bytes) != 0) return -1;
+            }
+        }
         return 0;
     }
 
     // device in/out, asynchronous on s
-    int run_device(const void* dx, size_t n, void* dy, size_t* n_out, cudaStream_t s) {
-        if (!committed && commit(1) != 0) return -1;
+    int run(const void* dx, size_t n, void* dy, size_t* n_out, cudaStream_t s) override {
+        if (ensure_committed() != 0) return -1;
         if (stages.empty()) { set_error("graph: no blocks"); return -1; }
-        // size the ring for this n
-        size_t m = n;
-        for (size_t k = 0; k + 1 < stages.size(); ++k) {
-            m = stages[k]->max_output(m);
-            size_t bytes = (m ? m : 1) * stages[k]->out_size;
-            int slot = (int)(k & 1);
-            if (bytes > ring[slot].capacity()) {
-                // a stage still in flight may be reading the old buffer
-                LRB_CHECK(cudaStreamSynchronize(s));
-                if (ring[slot].reserve(bytes) != 0) return -1;
-            }
-        }
+        if (reserve_ring(n, s) != 0) return -1;
         const void* in = dx;
         size_t cnt = n;
         for (size_t k = 0; k < stages.size(); ++k) {
             void* out = (k + 1 == stages.size()) ? dy : ring[k & 1].get();
             size_t no = 0;
-            if (timing) {
-                if (tcount.size() < stages.size()) { tev.resize(stages.size()); tcount.assign(stages.size(), 0); }
-                cudaEventRecord(timing_event(k, 2 * (size_t)tcount[k]), s);
-            }
+            timing_start(k, s);
             if (stages[k]->run(in, cnt, out, &no, s) != 0) return -1;
-            if (timing) { cudaEventRecord(timing_event(k, 2 * (size_t)tcount[k] + 1), s); tcount[k]++; }
+            timing_stop(k, s);
             in = out;
             cnt = no;
         }
@@ -276,10 +338,10 @@ struct Graph {
 
     // host in/out: pipelined H2D | kernels | D2H over two slots
     int run_host(const void* x, size_t n, void* y, size_t* n_out) {
-        if (!committed && commit(1) != 0) return -1;
+        if (ensure_committed() != 0) return -1;
         if (stages.empty()) { set_error("graph: no blocks"); return -1; }
         cudaStream_t s = ctx().stream;
-        const size_t isz = stages.front()->in_size, osz = stages.back()->out_size;
+        const size_t isz = in_size, osz = out_size;
         if (sc) return run_accumulate(x, n, y, n_out);
         if (n <= host_chunk) {
             // one chunk (every call of the reference's per-vector regime, pipe.lua:73): copy, kernels and copy back in
@@ -291,7 +353,7 @@ struct Graph {
             }
             size_t no = 0;
             if (n) LRB_CHECK(cudaMemcpyAsync(d_in[0].get(), x, n * isz, cudaMemcpyHostToDevice, s));
-            if (run_device(d_in[0].get(), n, d_out[0].get(), &no, s) != 0) return -1;
+            if (run(d_in[0].get(), n, d_out[0].get(), &no, s) != 0) return -1;
             if (no) LRB_CHECK(cudaMemcpyAsync(y, d_out[0].get(), no * osz, cudaMemcpyDeviceToHost, s));
             LRB_CHECK(cudaStreamSynchronize(s));
             *n_out = no;
@@ -314,7 +376,7 @@ struct Graph {
             LRB_CHECK(cudaStreamWaitEvent(s, ev_h2d[slot], 0));
             if (it >= 2) LRB_CHECK(cudaStreamWaitEvent(s, ev_d2h[slot], 0));          // d_out[slot] drained
             size_t no = 0;
-            if (run_device(d_in[slot].get(), nc, d_out[slot].get(), &no, s) != 0) return -1;
+            if (run(d_in[slot].get(), nc, d_out[slot].get(), &no, s) != 0) return -1;
             LRB_CHECK(cudaEventRecord(ev_comp[slot], s));
             LRB_CHECK(cudaStreamWaitEvent(s_d2h, ev_comp[slot], 0));
             if (no) LRB_CHECK(cudaMemcpyAsync((char*)y + produced * osz, d_out[slot].get(), no * osz, cudaMemcpyDeviceToHost, s_d2h));
@@ -332,12 +394,12 @@ struct Graph {
 
     // ---- super-chunk mode -------------------------------------------------------------------------------------
     int set_superchunk(size_t samples) {
-        if (!committed && commit(1) != 0) return -1;
+        if (ensure_committed() != 0) return -1;
         if (stages.empty()) { set_error("graph: no blocks"); return -1; }
         if (sc_pending[0] || sc_pending[1] || sc_fill) { set_error("graph: flush before changing the super-chunk size"); return -1; }
         free_superchunk();
         if (samples == 0) return 0;
-        const size_t isz = stages.front()->in_size, osz = stages.back()->out_size;
+        const size_t isz = in_size, osz = out_size;
         sc_outcap = max_output(samples) + 1;
         for (int i = 0; i < 2; ++i) {
             char* p = nullptr;
@@ -354,17 +416,17 @@ struct Graph {
     size_t sc_collect(int slot, char* y) {
         if (!sc_pending[slot]) return 0;
         if (!cuda_ok(cudaEventSynchronize(sc_done[slot]), "cudaEventSynchronize")) return (size_t)-1;
-        const size_t osz = stages.back()->out_size;
+        const size_t osz = out_size;
         if (sc_nout[slot]) memcpy(y, sc_hout[slot].get(), sc_nout[slot] * osz);
         sc_pending[slot] = false;
         return sc_nout[slot];
     }
     int sc_submit(int slot, size_t count) {
         cudaStream_t s = ctx().stream;
-        const size_t isz = stages.front()->in_size, osz = stages.back()->out_size;
+        const size_t isz = in_size, osz = out_size;
         size_t no = 0;
         LRB_CHECK(cudaMemcpyAsync(sc_din[slot].get(), sc_hin[slot].get(), count * isz, cudaMemcpyHostToDevice, s));
-        if (run_device(sc_din[slot].get(), count, sc_dout[slot].get(), &no, s) != 0) return -1;
+        if (run(sc_din[slot].get(), count, sc_dout[slot].get(), &no, s) != 0) return -1;
         if (no) LRB_CHECK(cudaMemcpyAsync(sc_hout[slot].get(), sc_dout[slot].get(), no * osz, cudaMemcpyDeviceToHost, s));
         LRB_CHECK(cudaEventRecord(sc_done[slot], s));
         sc_nout[slot] = no;
@@ -372,7 +434,7 @@ struct Graph {
         return 0;
     }
     int run_accumulate(const void* x, size_t n, void* y, size_t* n_out) {
-        const size_t isz = stages.front()->in_size, osz = stages.back()->out_size;
+        const size_t isz = in_size, osz = out_size;
         const char* xp = (const char*)x;
         char* yp = (char*)y;
         size_t produced = 0;
@@ -396,7 +458,7 @@ struct Graph {
     int flush(void* y, size_t* n_out) {
         *n_out = 0;
         if (!sc) return 0;
-        const size_t osz = stages.back()->out_size;
+        const size_t osz = out_size;
         char* yp = (char*)y;
         size_t produced = 0;
         size_t got = sc_collect(sc_cur ^ 1, yp);
@@ -425,7 +487,7 @@ struct Graph {
         if (ptrs.empty()) return 0;
         return launch_zero_segments(ptrs.data(), bytes.data(), (int)ptrs.size(), s);
     }
-    int reset() { return reset(ctx().stream); }
+    int reset() override { return reset(ctx().stream); }
 
     // ---- time-chunk sharding (SURVEY.md 8e) -------------------------------------------------------------------
     // total rate change in lowest terms: outputs per input = up / down
@@ -444,13 +506,13 @@ struct Graph {
     // input samples of left context a cold start needs so that the outputs equal the streaming ones to float32
     // resolution, rounded up to a whole number of output periods; < 0 when a stage's memory is unbounded
     long long halo() {
-        if (!committed && commit(1) != 0) return -1;
+        if (ensure_committed() != 0) return -1;
         double need = 0.0;                                   // at the input rate of the stage being visited
         for (size_t k = stages.size(); k-- > 0;) {
             unsigned bu, bd;
             stages[k]->rate(&bu, &bd);
             const long long mem = stages[k]->memory_in();
-            if (mem < 0) { set_error("graph: %s has unbounded memory, the stream cannot be cut", stages[k]->name); return -1; }
+            if (mem < 0) { set_error("graph: %s has unbounded memory, the stream cannot be cut", stages[k]->name.c_str()); return -1; }
             need = std::ceil(need * (double)bd / (double)bu) + (double)mem + 1.0;
         }
         unsigned long long up, down;
@@ -471,20 +533,18 @@ struct Graph {
     // (Ctx::lead_samples / lead_event); everything else starts at once, so the exchange overlaps the chunk's kernels.
     // A first stage that cannot do that makes the compute stream wait for the event (the exchange is then serial).
     // The last stage runs as two streaming calls -- the inputs that belong to the halo (their outputs go to a scratch
-    // buffer), then the rest straight into dy -- so dy receives exactly the chunk's outputs.  `head` is unused (kept in
-    // the C ABI for callers that built a second graph for the former head-piece scheme).
-    int run_shard(Graph& head, const void* dx, size_t halo_n, size_t n, uint64_t start, void* dy, size_t* n_out, cudaEvent_t halo_ready) {
-        (void)head;
-        if (!committed && commit(1) != 0) return -1;
+    // buffer), then the rest straight into dy -- so dy receives exactly the chunk's outputs.
+    int run_shard(const void* dx, size_t halo_n, size_t n, uint64_t start, void* dy, size_t* n_out, cudaEvent_t halo_ready) {
+        if (ensure_committed() != 0) return -1;
         if (stages.empty()) { set_error("graph: no blocks"); return -1; }
         cudaStream_t s = ctx().stream;
-        const size_t isz = stages.front()->in_size, osz = stages.back()->out_size;
+        const size_t isz = in_size, osz = out_size;
         unsigned long long up, down;
         total_rate(&up, &down);
         if (halo_n % down || start % down) { set_error("graph: halo and start must be multiples of %llu input samples", down); return -1; }
         if (halo_n == 0 || start == 0) {                     // the stream's first chunk: nothing to its left
             if (reset(s) != 0 || seek(start) != 0) return -1;
-            return run_device((const char*)dx + halo_n * isz, n, dy, n_out, s);
+            return run((const char*)dx + halo_n * isz, n, dy, n_out, s);
         }
         if (start < halo_n) { set_error("graph: chunk starts inside the halo"); return -1; }
         if (reset(s) != 0 || seek(start - halo_n) != 0) return -1;
@@ -505,18 +565,8 @@ struct Graph {
             LRB_CHECK(cudaStreamSynchronize(s));
             if (head_out.reserve((ho + 1) * osz) != 0) return -1;
         }
-        // ring for halo + n inputs
         const size_t n_tot = halo_n + n;
-        size_t m = n_tot;
-        for (size_t k = 0; k + 1 < K; ++k) {
-            m = stages[k]->max_output(m);
-            const size_t bytes = (m ? m : 1) * stages[k]->out_size;
-            const int slot = (int)(k & 1);
-            if (bytes > ring[slot].capacity()) {
-                LRB_CHECK(cudaStreamSynchronize(s));
-                if (ring[slot].reserve(bytes) != 0) return -1;
-            }
-        }
+        if (reserve_ring(n_tot, s) != 0) return -1;
         const bool overlap = halo_ready && K >= 2 && stages[0]->supports_lead_wait();
         if (halo_ready && !overlap) LRB_CHECK(cudaStreamWaitEvent(s, halo_ready, 0));
         const void* in = dx;
@@ -524,10 +574,7 @@ struct Graph {
         int rc = 0;
         for (size_t k = 0; k < K && rc == 0; ++k) {
             const bool last = k + 1 == K;
-            if (timing) {
-                if (tcount.size() < K) { tev.resize(K); tcount.assign(K, 0); }
-                cudaEventRecord(timing_event(k, 2 * (size_t)tcount[k]), s);
-            }
+            timing_start(k, s);
             if (k == 0 && overlap) { ctx().lead_samples = (long long)halo_n; ctx().lead_event = halo_ready; ctx().reserve_ctas = 4; }
             size_t no = 0;
             if (!last) {
@@ -549,15 +596,15 @@ struct Graph {
                 cnt = no;
             }
             if (k == 0) { ctx().lead_samples = 0; ctx().lead_event = nullptr; ctx().reserve_ctas = 0; }
-            if (timing) { cudaEventRecord(timing_event(k, 2 * (size_t)tcount[k] + 1), s); tcount[k]++; }
+            timing_stop(k, s);
         }
         if (rc != 0) return -1;
         *n_out = cnt;
         return 0;
     }
 
-    int seek(uint64_t idx) {
-        if (!committed && commit(1) != 0) return -1;
+    int seek(uint64_t idx) override {
+        if (ensure_committed() != 0) return -1;
         for (Block* b : stages) {
             if (b->seek(idx) != 0) return -1;
             idx = b->outputs_before(idx);
@@ -576,19 +623,11 @@ struct Graph {
 // the node launches in order on the library stream, one download per output, one synchronize.
 // This is what composites/wbfmstereodemodulator.lua:22-64 and amsynchronousdemodulator.lua:25-45 need on the device.
 // ---------------------------------------------------------------------------------------------------------------------
-void destroy_graph_handle(void* holder);      // delete (lrb200_graph_t*) -- defined behind the handle type below
-
 struct DagNode {
-    std::unique_ptr<Block> blk;
-    Graph* sub = nullptr;          // a committed linear run: lives inside `holder` (the caller's former handle, owned)
-    void* holder = nullptr;
+    std::unique_ptr<Block> blk;    // a block, or a committed linear Graph
     std::vector<int> in_refs;      // producer node * 4 + port, or -1 for the DAG input
     std::vector<DeviceBuffer> out_buf;
     std::vector<size_t> out_cnt;
-    int nout() const { return sub ? 1 : blk->num_outputs; }
-    size_t out_size(int port) const { return sub ? sub->stages.back()->out_size : blk->out_size_of(port); }
-    size_t in_size() const { return sub ? sub->stages.front()->in_size : blk->in_size; }
-    const char* name() const { return sub ? sub->desc.c_str() : blk->name; }
 };
 
 struct Dag {
@@ -598,50 +637,43 @@ struct Dag {
     size_t in_size = 0;
     std::string desc;
 
-    ~Dag() {
-        for (DagNode& nd : nodes)
-            if (nd.holder) destroy_graph_handle(nd.holder);
-    }
-
-    // on success the DAG owns blk (or holder); on failure the caller keeps it
-    int add(Block* blk, Graph* sub, void* holder, const int* refs, unsigned nin) {
+    // on success the DAG owns blk; on failure the caller keeps it
+    int add(Block* blk, const int* refs, unsigned nin) {
         DagNode nd;
-        nd.blk.reset(blk); nd.sub = sub; nd.holder = holder;
+        nd.blk.reset(blk);
         if (wire(nd, refs, nin) != 0) { nd.blk.release(); return -1; }
-        nd.out_buf.resize((size_t)nd.nout());
-        nd.out_cnt.assign((size_t)nd.nout(), 0);
+        nd.out_buf.resize((size_t)blk->num_outputs);
+        nd.out_cnt.assign((size_t)blk->num_outputs, 0);
         if (!desc.empty()) desc += " ; ";
-        desc += nd.name();
+        desc += blk->name;
         nodes.push_back(std::move(nd));
         return (int)nodes.size() - 1;
     }
 
     int wire(DagNode& nd, const int* refs, unsigned nin) {
-        const int want = nd.sub ? 1 : nd.blk->num_inputs;
-        if ((int)nin != want) { set_error("dag: %s takes %d input(s), got %u", nd.name(), want, nin); return -1; }
+        const Block& b = *nd.blk;
+        if ((int)nin != b.num_inputs) { set_error("dag: %s takes %d input(s), got %u", b.name.c_str(), b.num_inputs, nin); return -1; }
         for (unsigned i = 0; i < nin; ++i) {
             const int r = refs[i];
             size_t esz;
             if (r == -1) {
-                if (in_size && in_size != nd.in_size()) { set_error("dag: the input feeds nodes of different sample sizes"); return -1; }
-                in_size = nd.in_size();
+                if (in_size && in_size != b.in_size) { set_error("dag: the input feeds nodes of different sample sizes"); return -1; }
+                in_size = b.in_size;
                 esz = in_size;
             } else {
                 const int pn = r >> 2, pp = r & 3;
-                if (r < 0 || pn >= (int)nodes.size() || pp >= nodes[(size_t)pn].nout()) { set_error("dag: bad input reference %d", r); return -1; }
-                esz = nodes[(size_t)pn].out_size(pp);
+                if (r < 0 || pn >= (int)nodes.size() || pp >= nodes[(size_t)pn].blk->num_outputs) { set_error("dag: bad input reference %d", r); return -1; }
+                esz = nodes[(size_t)pn].blk->out_size_of(pp);
             }
-            if (esz != nd.in_size()) { set_error("dag: %zu-byte samples cannot feed %s (%zu-byte input)", esz, nd.name(), nd.in_size()); return -1; }
+            if (esz != b.in_size) { set_error("dag: %zu-byte samples cannot feed %s (%zu-byte input)", esz, b.name.c_str(), b.in_size); return -1; }
             nd.in_refs.push_back(r);
         }
         return 0;
     }
 
     int reset() {
-        for (DagNode& nd : nodes) {
-            if (nd.sub) { if (nd.sub->reset() != 0) return -1; }
-            else if (nd.blk->reset() != 0) return -1;
-        }
+        for (DagNode& nd : nodes)
+            if (nd.blk->reset() != 0) return -1;
         return 0;
     }
 
@@ -660,15 +692,16 @@ struct Dag {
                 const int r = nd.in_refs[i];
                 const void* p = r == -1 ? d_in.get() : nodes[(size_t)(r >> 2)].out_buf[(size_t)(r & 3)].get();
                 const size_t c = r == -1 ? n : nodes[(size_t)(r >> 2)].out_cnt[(size_t)(r & 3)];
-                if (i && c != cnt) { set_error("dag: %s received inputs of different lengths (%zu, %zu)", nd.name(), cnt, c); return -1; }
+                if (i && c != cnt) { set_error("dag: %s received inputs of different lengths (%zu, %zu)", nd.blk->name.c_str(), cnt, c); return -1; }
                 cnt = c;
                 ins.push_back(p);
             }
-            const size_t mo = nd.sub ? nd.sub->max_output(cnt) : nd.blk->max_output(cnt);
+            const int nout = nd.blk->num_outputs;
+            const size_t mo = nd.blk->max_output(cnt);
             void* outs[4];                 // a port is two bits of a reference
-            for (int o = 0; o < nd.nout(); ++o) {
+            for (int o = 0; o < nout; ++o) {
                 DeviceBuffer& buf = nd.out_buf[(size_t)o];
-                const size_t bytes = (mo ? mo : 1) * nd.out_size(o);
+                const size_t bytes = (mo ? mo : 1) * nd.blk->out_size_of(o);
                 if (bytes > buf.capacity()) {
                     LRB_CHECK(cudaStreamSynchronize(s));
                     if (buf.reserve(bytes) != 0) return -1;
@@ -676,18 +709,14 @@ struct Dag {
                 outs[o] = buf.get();
             }
             size_t no = 0;
-            if (nd.sub) {
-                if (nd.sub->run_device(ins[0], cnt, outs[0], &no, s) != 0) return -1;
-            } else {
-                if (nd.blk->run_multi(ins.data(), (int)ins.size(), cnt, outs, nd.nout(), &no, s) != 0) return -1;
-            }
-            for (int o = 0; o < nd.nout(); ++o) nd.out_cnt[(size_t)o] = no;
+            if (nd.blk->run_multi(ins.data(), (int)ins.size(), cnt, outs, nout, &no, s) != 0) return -1;
+            for (int o = 0; o < nout; ++o) nd.out_cnt[(size_t)o] = no;
         }
         for (size_t k = 0; k < outputs.size(); ++k) {
             const DagNode& nd = nodes[(size_t)(outputs[k] >> 2)];
             const int port = outputs[k] & 3;
             const size_t c = nd.out_cnt[(size_t)port];
-            if (c) LRB_CHECK(cudaMemcpyAsync(y[k], nd.out_buf[(size_t)port].get(), c * nd.out_size(port), cudaMemcpyDeviceToHost, s));
+            if (c) LRB_CHECK(cudaMemcpyAsync(y[k], nd.out_buf[(size_t)port].get(), c * nd.blk->out_size_of(port), cudaMemcpyDeviceToHost, s));
             n_out[k] = c;
         }
         LRB_CHECK(cudaStreamSynchronize(s));
@@ -699,30 +728,31 @@ struct Dag {
 
 using namespace lrb;
 
-struct lrb200_graph_s { Graph g; };
+struct lrb200_graph_s { std::unique_ptr<Graph> g; };
 struct lrb200_dag_s { Dag d; };
-namespace lrb { void destroy_graph_handle(void* holder) { delete static_cast<lrb200_graph_s*>(holder); } }
 
 extern "C" {
 
 lrb200_graph_t* lrb200_graph_create(void) {
     if (lrb200_device_count() <= 0) { set_error("no CUDA device available; libluaradio_b200 has no CPU fallback"); return nullptr; }
     if (ctx().device < 0 && lrb200_init(0) != 0) return nullptr;
-    lrb200_graph_t* g = new (std::nothrow) lrb200_graph_s();
+    std::unique_ptr<Graph> impl(new (std::nothrow) Graph());
+    lrb200_graph_t* g = impl ? new (std::nothrow) lrb200_graph_s{std::move(impl)} : nullptr;
     if (!g) set_error("out of memory");
     return g;
 }
 
 int lrb200_graph_append(lrb200_graph_t* g, lrb200_block_t* q) {
     if (!g || !q || !q->impl) { set_error("graph_append: null handle"); return -1; }
-    if (!q->impl->dev_ptrs) { set_error("graph_append: block %s was not created with LRB200_DEVICE", q->impl->name); return -1; }
-    if (!g->g.blocks.empty() && g->g.blocks.back()->out_size != q->impl->in_size) {
-        set_error("graph_append: %s (out %zu B) cannot feed %s (in %zu B)", g->g.blocks.back()->name,
-                  g->g.blocks.back()->out_size, q->impl->name, q->impl->in_size);
+    if (!q->impl->dev_ptrs) { set_error("graph_append: block %s was not created with LRB200_DEVICE", q->impl->name.c_str()); return -1; }
+    Blocks& blocks = g->g->blocks;
+    if (!blocks.empty() && blocks.back()->out_size != q->impl->in_size) {
+        set_error("graph_append: %s (out %zu B) cannot feed %s (in %zu B)", blocks.back()->name.c_str(),
+                  blocks.back()->out_size, q->impl->name.c_str(), q->impl->in_size);
         return -1;
     }
-    g->g.blocks.emplace_back(q->impl);
-    g->g.committed = false;
+    blocks.emplace_back(q->impl);
+    g->g->committed = false;
     q->impl = nullptr;          // ownership moves to the graph
     delete q;
     return 0;
@@ -730,13 +760,13 @@ int lrb200_graph_append(lrb200_graph_t* g, lrb200_block_t* q) {
 
 int lrb200_graph_commit(lrb200_graph_t* g, int fuse) {
     if (!g) { set_error("null graph"); return -1; }
-    return g->g.commit(fuse);
+    return g->g->commit(fuse);
 }
 
 int lrb200_graph_execute(lrb200_graph_t* g, const void* x, size_t n, void* y, size_t* n_out) {
     if (!g) { set_error("null graph"); return -1; }
     size_t no = 0;
-    int rc = g->g.run_host(x, n, y, &no);
+    int rc = g->g->run_host(x, n, y, &no);
     if (n_out) *n_out = no;
     return rc;
 }
@@ -744,97 +774,96 @@ int lrb200_graph_execute(lrb200_graph_t* g, const void* x, size_t n, void* y, si
 int lrb200_graph_execute_device(lrb200_graph_t* g, const void* dx, size_t n, void* dy, size_t* n_out) {
     if (!g) { set_error("null graph"); return -1; }
     size_t no = 0;
-    int rc = g->g.run_device(dx, n, dy, &no, ctx().stream);
+    int rc = g->g->run(dx, n, dy, &no, ctx().stream);
     if (n_out) *n_out = no;
     return rc;
 }
 
 size_t lrb200_graph_max_output(const lrb200_graph_t* g, size_t n) {
     if (!g) return 0;
-    lrb200_graph_t* gg = const_cast<lrb200_graph_t*>(g);
-    if (!gg->g.committed && gg->g.commit(1) != 0) return 0;
+    Graph& gr = *g->g;
+    if (gr.ensure_committed() != 0) return 0;
     // super-chunk mode: one call may hand back the results of the slots completed while n samples were appended
-    if (gg->g.sc) return (n / gg->g.sc + 2) * gg->g.sc_outcap;
-    return gg->g.max_output(n);
+    if (gr.sc) return (n / gr.sc + 2) * gr.sc_outcap;
+    return gr.max_output(n);
 }
 
 int lrb200_graph_set_superchunk(lrb200_graph_t* g, size_t samples) {
     if (!g) { set_error("null graph"); return -1; }
-    return g->g.set_superchunk(samples);
+    return g->g->set_superchunk(samples);
 }
 
 int lrb200_graph_flush(lrb200_graph_t* g, void* y, size_t* n_out) {
     if (!g) { set_error("null graph"); return -1; }
     size_t no = 0;
-    int rc = g->g.flush(y, &no);
+    int rc = g->g->flush(y, &no);
     if (n_out) *n_out = no;
     return rc;
 }
 
 long long lrb200_graph_halo(lrb200_graph_t* g) {
     if (!g) { set_error("null graph"); return -1; }
-    return g->g.halo();
+    return g->g->halo();
 }
 
 int lrb200_graph_execute_shard(lrb200_graph_t* g, lrb200_graph_t* g_head, const void* dx, size_t halo, size_t n,
                                uint64_t start, void* dy, size_t* n_out, void* halo_ready_event) {
     if (!g) { set_error("null graph"); return -1; }
     size_t no = 0;
-    int rc = g->g.run_shard(g_head ? g_head->g : g->g, dx, halo, n, start, dy, &no, (cudaEvent_t)halo_ready_event);
+    (void)g_head;
+    int rc = g->g->run_shard(dx, halo, n, start, dy, &no, (cudaEvent_t)halo_ready_event);
     if (n_out) *n_out = no;
     return rc;
 }
 
 int lrb200_graph_reset(lrb200_graph_t* g) {
     if (!g) { set_error("null graph"); return -1; }
-    return g->g.reset();
+    return g->g->reset();
 }
 
 int lrb200_graph_seek(lrb200_graph_t* g, uint64_t sample_index) {
     if (!g) { set_error("null graph"); return -1; }
-    return g->g.seek(sample_index);
+    return g->g->seek(sample_index);
 }
 
 int lrb200_graph_num_stages(const lrb200_graph_t* g) {
     if (!g) return 0;
-    lrb200_graph_t* gg = const_cast<lrb200_graph_t*>(g);
-    if (!gg->g.committed && gg->g.commit(1) != 0) return -1;
-    return (int)gg->g.stages.size();
+    if (g->g->ensure_committed() != 0) return -1;
+    return (int)g->g->stages.size();
 }
 
 const char* lrb200_graph_describe(const lrb200_graph_t* g) {
     if (!g) return "";
-    lrb200_graph_t* gg = const_cast<lrb200_graph_t*>(g);
-    if (!gg->g.committed && gg->g.commit(1) != 0) return "";
-    return gg->g.desc.c_str();
+    if (g->g->ensure_committed() != 0) return "";
+    return g->g->name.c_str();
 }
 
 const char* lrb200_graph_stage_name(const lrb200_graph_t* g, int stage) {
     if (!g) return "";
-    lrb200_graph_t* gg = const_cast<lrb200_graph_t*>(g);
-    if (!gg->g.committed && gg->g.commit(1) != 0) return "";
-    if (stage < 0 || stage >= (int)gg->g.stages.size()) return "";
-    return gg->g.stages[stage]->name;
+    Graph& gr = *g->g;
+    if (gr.ensure_committed() != 0) return "";
+    if (stage < 0 || stage >= (int)gr.stages.size()) return "";
+    return gr.stages[stage]->name.c_str();
 }
 
 int lrb200_graph_set_timing(lrb200_graph_t* g, int enable) {
     if (!g) { set_error("null graph"); return -1; }
-    g->g.timing = enable != 0;
+    g->g->timing = enable != 0;
     return 0;
 }
 
 double lrb200_graph_stage_time_ms(lrb200_graph_t* g, int stage, int* executions) {
     if (executions) *executions = 0;
-    if (!g || stage < 0 || stage >= (int)g->g.tcount.size()) return 0.0;
+    if (!g || stage < 0 || stage >= (int)g->g->tcount.size()) return 0.0;
     if (cudaStreamSynchronize(ctx().stream) != cudaSuccess) return 0.0;
     double total = 0.0;
-    int cnt = g->g.tcount[stage];
+    int cnt = g->g->tcount[stage];
     for (int i = 0; i < cnt; ++i) {
         float ms = 0.f;
-        if (cudaEventElapsedTime(&ms, g->g.tev[stage][2 * i], g->g.tev[stage][2 * i + 1]) == cudaSuccess) total += ms;
+        if (cudaEventElapsedTime(&ms, g->g->tev[stage][2 * i], g->g->tev[stage][2 * i + 1]) == cudaSuccess) total += ms;
     }
     if (executions) *executions = cnt;
-    g->g.tcount[stage] = 0;
+    g->g->tcount[stage] = 0;
     return total;
 }
 
@@ -851,8 +880,8 @@ lrb200_dag_t* lrb200_dag_create(void) {
 
 int lrb200_dag_add_block(lrb200_dag_t* d, lrb200_block_t* q, const int* inputs, unsigned num_inputs) {
     if (!d || !q || !q->impl || (!inputs && num_inputs)) { set_error("dag_add_block: null argument"); return -1; }
-    if (!q->impl->dev_ptrs) { set_error("dag_add_block: block %s was not created with LRB200_DEVICE", q->impl->name); return -1; }
-    const int id = d->d.add(q->impl, nullptr, nullptr, inputs, num_inputs);
+    if (!q->impl->dev_ptrs) { set_error("dag_add_block: block %s was not created with LRB200_DEVICE", q->impl->name.c_str()); return -1; }
+    const int id = d->d.add(q->impl, inputs, num_inputs);
     if (id < 0) return -1;
     q->impl = nullptr;          // ownership moves to the DAG
     delete q;
@@ -861,16 +890,20 @@ int lrb200_dag_add_block(lrb200_dag_t* d, lrb200_block_t* q, const int* inputs, 
 
 int lrb200_dag_add_graph(lrb200_dag_t* d, lrb200_graph_t* g, int input) {
     if (!d || !g) { set_error("dag_add_graph: null argument"); return -1; }
-    if (!g->g.committed && g->g.commit(1) != 0) return -1;
-    if (g->g.stages.empty()) { set_error("dag_add_graph: empty graph"); return -1; }
-    return d->d.add(nullptr, &g->g, g, &input, 1);       // on success the handle belongs to the DAG
+    if (g->g->ensure_committed() != 0) return -1;
+    if (g->g->stages.empty()) { set_error("dag_add_graph: empty graph"); return -1; }
+    const int id = d->d.add(g->g.get(), &input, 1);
+    if (id < 0) return -1;
+    g->g.release();             // ownership moves to the DAG
+    delete g;
+    return id;
 }
 
 int lrb200_dag_set_outputs(lrb200_dag_t* d, const int* outputs, unsigned num_outputs) {
     if (!d || !outputs || !num_outputs) { set_error("dag_set_outputs: null argument"); return -1; }
     for (unsigned k = 0; k < num_outputs; ++k) {
         const int r = outputs[k];
-        if (r < 0 || (r >> 2) >= (int)d->d.nodes.size() || (r & 3) >= d->d.nodes[(size_t)(r >> 2)].nout()) { set_error("dag_set_outputs: bad reference %d", r); return -1; }
+        if (r < 0 || (r >> 2) >= (int)d->d.nodes.size() || (r & 3) >= d->d.nodes[(size_t)(r >> 2)].blk->num_outputs) { set_error("dag_set_outputs: bad reference %d", r); return -1; }
     }
     d->d.outputs.assign(outputs, outputs + num_outputs);
     return 0;
@@ -885,7 +918,7 @@ size_t lrb200_dag_max_output(const lrb200_dag_t* d, unsigned output, size_t n) {
     if (!d || output >= d->d.outputs.size()) return 0;
     // conservative: no node here produces more samples than its input times the interpolation factors on the way
     size_t m = n;
-    for (const DagNode& nd : d->d.nodes) { const size_t c = nd.sub ? nd.sub->max_output(n) : nd.blk->max_output(n); if (c > m) m = c; }
+    for (const DagNode& nd : d->d.nodes) { const size_t c = nd.blk->max_output(n); if (c > m) m = c; }
     return m;
 }
 

@@ -147,14 +147,7 @@ const FmtInfo FORMATS[] = {
 
 struct IqConvBlock : Block {
     FmtInfo info;
-    std::string label;
-    explicit IqConvBlock(const FmtInfo& f, bool dev) : info(f) {
-        label = std::string("iqconv(") + f.name + ")";
-        name = label.c_str();
-        in_size = (size_t)2 * f.bytes;
-        out_size = 8;
-        dev_ptrs = dev;
-    }
+    explicit IqConvBlock(const FmtInfo& f, bool dev) : Block(std::string("iqconv(") + f.name + ")", (size_t)2 * f.bytes, 8, dev), info(f) {}
     int run(const void* dx, size_t n, void* dy, size_t* n_out, cudaStream_t s) override {
         *n_out = n;
         consumed += n;
@@ -288,14 +281,10 @@ struct FileConvBlock : Block {
     FmtInfo info;
     bool to_file;             // true: float -> raw (sinks); false: raw -> float (RealFileSource)
     int comps;                // components per sample (1 real, 2 complex)
-    std::string label;
-    FileConvBlock(const FmtInfo& f, bool to_file_, int comps_, bool dev) : info(f), to_file(to_file_), comps(comps_) {
-        label = std::string(to_file ? (comps == 2 ? "iqsink(" : "realsink(") : "realconv(") + f.name + ")";
-        name = label.c_str();
-        in_size = to_file ? 4 * (size_t)comps : (size_t)f.bytes * comps;
-        out_size = to_file ? (size_t)f.bytes * comps : 4 * (size_t)comps;
-        dev_ptrs = dev;
-    }
+    FileConvBlock(const FmtInfo& f, bool to_file_, int comps_, bool dev)
+        : Block(std::string(to_file_ ? (comps_ == 2 ? "iqsink(" : "realsink(") : "realconv(") + f.name + ")",
+                to_file_ ? 4 * (size_t)comps_ : (size_t)f.bytes * comps_, to_file_ ? (size_t)f.bytes * comps_ : 4 * (size_t)comps_, dev),
+          info(f), to_file(to_file_), comps(comps_) {}
     int run(const void* dx, size_t n, void* dy, size_t* n_out, cudaStream_t s) override {
         *n_out = n;
         consumed += n;

@@ -356,12 +356,10 @@ level_kernel(const T* __restrict__ x, long long n, T* __restrict__ y, LevelParam
 }  // namespace
 
 // ---------------------------------------------------------------------------------------------
-LevelBlock::LevelBlock(bool agc_, double power_alpha, double gain_alpha, double target, double threshold, bool cplx, bool dev) {
+LevelBlock::LevelBlock(bool agc_, double power_alpha, double gain_alpha, double target, double threshold, bool cplx, bool dev)
+    : Block(agc_ ? (cplx ? "agc_cc" : "agc_rr") : (cplx ? "powersquelch_cc" : "powersquelch_rr"), cplx ? 8 : 4, cplx ? 8 : 4, dev) {
     agc = agc_;
     complex_data = cplx;
-    name = agc ? (cplx ? "agc_cc" : "agc_rr") : (cplx ? "powersquelch_cc" : "powersquelch_rr");
-    in_size = out_size = cplx ? 8 : 4;
-    dev_ptrs = dev;
     pa = power_alpha;
     ga = gain_alpha;
     T = target;

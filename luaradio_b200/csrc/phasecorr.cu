@@ -229,10 +229,7 @@ __global__ void __launch_bounds__(PC_THREADS, 3) pc_apply_kernel(PcParams P) {
 }  // namespace
 
 // ---------------------------------------------------------------------------------------------
-PhaseCorrectorBlock::PhaseCorrectorBlock(unsigned num_samples, unsigned sample_interval, bool dev) {
-    name = "phasecorr";
-    in_size = out_size = 8;
-    dev_ptrs = dev;
+PhaseCorrectorBlock::PhaseCorrectorBlock(unsigned num_samples, unsigned sample_interval, bool dev) : Block("phasecorr", 8, 8, dev) {
     N = num_samples;
     I = sample_interval;
 }

@@ -365,11 +365,8 @@ int grid_for(long long n) {
 }  // namespace
 
 // ---------------------------------------------------------------------------------------------
-ScaleBlock::ScaleBlock(float re, float im, bool cdata, bool cconst, bool dev) : cre(re), cim(im), complex_data(cdata), complex_const(cconst) {
-    name = "mulconst";
-    in_size = out_size = cdata ? 8 : 4;
-    dev_ptrs = dev;
-}
+ScaleBlock::ScaleBlock(float re, float im, bool cdata, bool cconst, bool dev)
+    : Block("mulconst", cdata ? 8 : 4, cdata ? 8 : 4, dev), cre(re), cim(im), complex_data(cdata), complex_const(cconst) {}
 int ScaleBlock::run(const void* dx, size_t n, void* dy, size_t* n_out, cudaStream_t s) {
     *n_out = n;
     consumed += n;
@@ -383,12 +380,7 @@ int ScaleBlock::run(const void* dx, size_t n, void* dy, size_t* n_out, cudaStrea
     return 0;
 }
 
-UpsampleBlock::UpsampleBlock(unsigned factor, unsigned elem, bool dev) {
-    name = "upsample";
-    in_size = out_size = elem;
-    dev_ptrs = dev;
-    L = (int)factor;
-}
+UpsampleBlock::UpsampleBlock(unsigned factor, unsigned elem, bool dev) : Block("upsample", elem, elem, dev) { L = (int)factor; }
 int UpsampleBlock::run(const void* dx, size_t n, void* dy, size_t* n_out, cudaStream_t s) {
     const long long no = (long long)n * L;
     *n_out = (size_t)no;
@@ -403,12 +395,10 @@ int UpsampleBlock::run(const void* dx, size_t n, void* dy, size_t* n_out, cudaSt
 
 // ---------------------------------------------------------------------------------------------
 InterpFirBlock::InterpFirBlock(bool cdata, const float* taps_host, int ntaps, int interp, int decim, bool has_scale_, float scale_, bool dev)
-    : complex_data(cdata), L(interp), D(decim), M(ntaps), has_scale(has_scale_), scale(scale_) {
-    label = std::string(has_scale ? "mulconst+" : "") + "upsample+fir" + (D > 1 ? "+down" : "") + "(" + std::to_string(M) + ",x" +
-            std::to_string(L) + (D > 1 ? "/" + std::to_string(D) : "") + ")";
-    name = label.c_str();
-    in_size = out_size = cdata ? 8 : 4;
-    dev_ptrs = dev;
+    : Block(std::string(has_scale_ ? "mulconst+" : "") + "upsample+fir" + (decim > 1 ? "+down" : "") + "(" + std::to_string(ntaps) +
+                ",x" + std::to_string(interp) + (decim > 1 ? "/" + std::to_string(decim) : "") + ")",
+            cdata ? 8 : 4, cdata ? 8 : 4, dev),
+      complex_data(cdata), L(interp), D(decim), M(ntaps), has_scale(has_scale_), scale(scale_) {
     h_taps.assign(taps_host, taps_host + ntaps);
     Hn = (M + L - 1) / L;
 }

@@ -962,16 +962,13 @@ struct TunerBlock : Block {
     int cur = 0, pcur = 0;
     bool disc = false;
     float gain = 1.f;
-    std::string label;
 
-    TunerBlock(std::unique_ptr<PolyTaps>&& p, float disc_gain) : M(p->M), D(p->D), pt(std::move(p)) {
+    TunerBlock(std::unique_ptr<PolyTaps>&& p, float disc_gain)
+        : Block(std::string(disc_gain != 0.0f ? "tuner+discrim(" : "tuner(") + std::to_string(p->M) + ",/" + std::to_string(p->D) + ")",
+                8, disc_gain != 0.0f ? 4 : 8, true),
+          M(p->M), D(p->D), pt(std::move(p)) {
         disc = disc_gain != 0.0f;
         gain = disc_gain;
-        in_size = 8;
-        out_size = disc ? 4 : 8;
-        dev_ptrs = true;
-        label = std::string(disc ? "tuner+discrim(" : "tuner(") + std::to_string(M) + ",/" + std::to_string(D) + ")";
-        name = label.c_str();
     }
     int init() override {
         return carry(d_hist, (size_t)(M > 1 ? M - 1 : 1) * 8, cur) != 0 || carry(d_prev, 8, pcur) != 0 ? -1 : 0;
