@@ -195,7 +195,7 @@ lrb200_block_t* lrb200_upsample_create(unsigned factor, unsigned elem_size, unsi
  * lrb200_delay_create replaces DelayBlock:process (radio/blocks/signal/delay.lua:26-60): y[n] = x[n - num_samples],
  * zeros first, the last num_samples inputs carried.
  * lrb200_psd_create replaces spectrum_utils.PSD:compute (radio/utilities/spectrum_utils.lua:524-642), the engine of the
- * spectrum sinks: every whole frame of num_samples inputs (power of two <= 4096) is multiplied by `window`
+ * spectrum sinks: every whole frame of num_samples inputs (power of two, 2..2^20) is multiplied by `window`
  * (window_utils.window(N, type, true)), transformed, and |X_k|^2 / scale (scale = sample_rate * window energy) is written,
  * as 10*log10 of it when logarithmic != 0; n must be a multiple of num_samples.
  * lrb200_pll_create replaces PLLBlock:process (radio/blocks/signal/pll.lua:113-170): loop constants from

@@ -8,7 +8,7 @@
 //   PSD          radio/utilities/spectrum_utils.lua:524-642: window -> DFT -> |X_k|^2 / (rate * window energy) [-> 10 log10]
 //
 // All HBM-streaming kernels (128-bit accesses where the pointers allow); the PSD runs one CTA per frame with the
-// transform in shared memory (frames of up to 4096 points, power of two).
+// transform in shared memory (frames of up to 4096 points, power of two; longer frames, up to 2^20, in psd_long.cu).
 #include "../../include/lrb200.h"
 #include "common.cuh"
 #include "blocks.h"
@@ -465,17 +465,20 @@ struct PsdBlock : Block {
     int N, logN;
     bool cplx, logarithmic;
     float inv_scale;
+    double scale;
     std::vector<float> h_window;
     DeviceBuffer d_window;
     DeviceBuffer d_tw;
     DeviceBuffer d_tw1024;           // N == 1024: inter-pass twiddles of the register-resident transform
-    PsdBlock(int N_, const float* window, double scale, bool log_, bool cplx_, bool dev)
-        : Block("psd", cplx_ ? 8 : 4, 4, dev), N(N_), cplx(cplx_), logarithmic(log_), inv_scale((float)(1.0 / scale)) {
+    PsdLong plong;                   // N > 4096 (psd_long.cu)
+    PsdBlock(int N_, const float* window, double scale_, bool log_, bool cplx_, bool dev)
+        : Block("psd", cplx_ ? 8 : 4, 4, dev), N(N_), cplx(cplx_), logarithmic(log_), inv_scale((float)(1.0 / scale_)), scale(scale_) {
         logN = 0;
         while ((1 << logN) < N) ++logN;
         h_window.assign(window, window + N);
     }
     int init() override {
+        if (N >= PSD_LONG_MIN) return d_window.upload(h_window.data(), sizeof(float) * (size_t)N) != 0 ? -1 : plong.init(N);
         std::vector<float2> tw((size_t)N / 2 + 1);
         for (int k = 0; k < N / 2; ++k)
             tw[(size_t)k] = make_float2((float)std::cos(2 * M_PI * k / N), (float)(-std::sin(2 * M_PI * k / N)));
@@ -498,6 +501,11 @@ struct PsdBlock : Block {
         if (n == 0) return 0;
         const size_t frames = n / (size_t)N;
         if (frames > 2147483647u) { set_error("psd: too many frames in one call"); return -1; }
+        if (N >= PSD_LONG_MIN) {
+            if (plong.run(dx, d_window.as<float>(), (float*)dy, (long long)frames, cplx, 1.0 / scale, logarithmic, s) != 0) return -1;
+            consumed += n;
+            return 0;
+        }
         if (N == 1024) {
             constexpr size_t smem = sizeof(float2) * (1024 + 512 + PS_WARPS * 32 * PS_XSTRIDE);
             long long ctas = ((long long)frames + PS_WARPS - 1) / PS_WARPS;
@@ -560,8 +568,8 @@ lrb200_block_t* lrb200_delay_create(unsigned num_samples, unsigned elem_size, un
 lrb200_block_t* lrb200_psd_create(unsigned num_samples, const float32_t* window, double scale, unsigned logarithmic,
                                   unsigned complex_data, unsigned flags) {
     if (ctx().device < 0 && lrb200_init(0) != 0) return nullptr;
-    if (num_samples < 2 || num_samples > 4096 || (num_samples & (num_samples - 1))) {
-        set_error("psd: the frame length must be a power of two in 2..4096 (got %u)", num_samples);
+    if (num_samples < 2 || num_samples > (unsigned)PSD_LONG_MAX || (num_samples & (num_samples - 1))) {
+        set_error("psd: the frame length must be a power of two in 2..%d (got %u)", PSD_LONG_MAX, num_samples);
         return nullptr;
     }
     if (!window) { set_error("psd: missing window"); return nullptr; }

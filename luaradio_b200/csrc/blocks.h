@@ -264,6 +264,19 @@ struct PhaseCorrectorBlock : Block {
     long long memory_in() const override;
 };
 
+// psd_long.cu: the PSD transform of frames of 8192 <= N <= 2^20 points (power of two) for PsdBlock
+constexpr int PSD_LONG_MIN = 8192, PSD_LONG_MAX = 1 << 20;
+constexpr int PSD_LONG_SINGLE_MAX = 16384;           // one CTA per frame up to here, two passes through scratch above
+constexpr long long PSD_LONG_BATCH = 1LL << 25;      // samples per two-pass batch: 256 MiB of complex64 scratch
+struct PsdLong {
+    int N = 0;
+    DeviceBuffer d_tw;                               // twiddle tables (psd_long.cu)
+    DeviceBuffer d_scratch;                          // two-pass form: the column pass's output
+    int init(int N);
+    int run(const void* x, const float* window, float* y, long long frames, bool cplx, double inv_scale, bool logarithmic,
+            cudaStream_t s);
+};
+
 }  // namespace lrb
 
 // the opaque public handle

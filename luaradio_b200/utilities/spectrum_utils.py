@@ -4,8 +4,10 @@ reference's spectrum sinks (gnuplotspectrum / gnuplotwaterfall call PSD:compute 
     psd = PSD(num_samples, complex_input, window_type="hamming", sample_rate=2, logarithmic=True)
     out = psd.compute(samples)          # any whole number of num_samples-frames -> as many PSD frames
 
-window -> DFT -> |X_k|^2 / (sample_rate * window energy) [-> 10*log10], frames of a power of two up to 4096 points, one
-CTA per frame (lrb200_psd_create).  fftshift() is the host-side reordering of spectrum_utils.lua:646-667."""
+window -> DFT -> |X_k|^2 / (sample_rate * window energy) [-> 10*log10], frames of a power of two from 2 to 2^20 points
+(lrb200_psd_create): up to 16384 points one CTA per frame, longer frames in two passes through a device scratch buffer.
+Other even lengths, which the reference accepts, raise.  fftshift() is the host-side reordering of
+spectrum_utils.lua:646-667."""
 import ctypes
 
 import numpy as np
