@@ -84,8 +84,33 @@ inline long long decay_samples(double c) {        // samples until |c|^k < 1e-12
     return (long long)std::ceil(std::log(1e-12) / std::log(a)) + 1;
 }
 
-struct FirFast;   // overlap-save plan (fir_fft.cu)
+// fir_fft.cu: a FIR's overlap-save plan, made at creation (*out stays null when no overlap-save kernel covers the
+// shape), and the two ways to run a call through it.  0, or -1 with the error set.
+constexpr int FIR_FFT_N = 1024;
+constexpr int FFT_MAX_TAPS = 513;       // L >= 512: at most half of every block is overlap
+struct FirFast {
+    int in_mode = 0;           // 0: complex in; 1: real in, two blocks packed per transform (rrrf); 2: Hilbert
+    int M = 0, D = 1;
+    int nparts = 1;            // > 1: uniformly partitioned overlap-save for filters longer than one block allows
+    int part_taps = 0;         // taps per partition (M unless partitioned)
+    bool rotate = false;       // a translator of rot_fix turns per sample fused in front
+    uint64_t rot_fix = 0;
+    DeviceBuffer d_H;          // nparts tap spectra, FIR_FFT_N each
+    DeviceBuffer d_tw;
+    DeviceBuffer d_E;
+    int block_len() const { return FIR_FFT_N - (part_taps - 1); }     // L: outputs per block
+};
+int fir_fast_prepare(FirKind kind, const void* taps, int M, int D, bool rotate, uint64_t rot_fix,
+                     std::unique_ptr<FirFast>* out);
+int launch_overlap_save(const FirFast& f, const void* x, const void* hist, long long n, void* y, long long first,
+                        uint64_t g0, cudaStream_t s);
+int launch_delay_line(const FirFast& f, const void* x, const void* hist, long long n, void* y, cudaStream_t s);
+
 struct PolyTaps;  // polyphase decimator taps (tuner.cu)
+
+// The kernel a FirBlock call runs: register-tiled polyphase (tuner.cu), generic-shape polyphase (poly_generic.cu),
+// single-block overlap-save or partitioned delay line (fir_fft.cu), catch-all direct form (fir_direct.cu)
+enum class FirPath { Polyphase, PolyGeneric, OverlapSave, DelayLine, Direct };
 
 struct FirBlock : Block {
     FirKind kind;
@@ -99,9 +124,10 @@ struct FirBlock : Block {
     bool rotate = false;              // fused FrequencyTranslator in front (graph fusion; FFT path only)
     double rot_turns = 0.0;
     uint64_t rot_fix = 0;
-    FirFast* fast = nullptr;          // owned; deleted in fir_fft.cu, where the type is complete
+    // the kernels that cover this block, decided at init: overlap-save plan, polyphase taps, generic polyphase shape
+    std::unique_ptr<FirFast> fast;
     PolyTaps* poly = nullptr;
-    bool gen_poly = false;            // poly_generic.cu covers this (kind, M, D)
+    bool gen_poly = false;
     // output-rate pole fused behind a real polyphase decimator (graph rewrite of FIR -> IIR1 -> Downsampler)
     bool has_pole = false;
     float pole_c = 0.f;
@@ -119,13 +145,12 @@ struct FirBlock : Block {
     uint64_t outputs_before(uint64_t idx) const override { return (idx + D - 1) / D; }
     long long memory_in() const override;
     void rate(unsigned* up, unsigned* down) const override { *up = 1; *down = (unsigned)D; }
-    bool supports_lead_wait() const override { return poly != nullptr && algo != 2 /* LRB200_FIR_FFT */ && !rotate; }
-    bool state_only_on_side_stream() const override { return poly != nullptr && algo != 2 && !rotate; }
-    // fast paths (fir_fft.cu): fast_run returns 1 if it handled the call, 0 to fall back, <0 on error
-    int fast_init();
-    int fast_run(const void* dx, size_t n, void* dy, long long first, long long n_out, cudaStream_t s);
+    bool supports_lead_wait() const override { return always_polyphase(); }
+    bool state_only_on_side_stream() const override { return always_polyphase(); }
     int set_algorithm(int a);
-    int effective_algorithm() const;
+    FirPath path(size_t n) const;     // the kernel a call of n inputs runs
+    bool always_polyphase() const { return poly != nullptr && algo != LRB200_FIR_FFT; }    // path(n) for every n
+    int effective_algorithm() const;  // path() of a long call as LRB200_FIR_DIRECT / FFT (lrb200_fir_get_algorithm)
 };
 
 struct RotatorBlock : Block {
@@ -297,19 +322,18 @@ lrb200_block_s* create_block(unsigned flags, A&&... args) {
     return block_handle(make_block<B>(std::forward<A>(args)..., (flags & LRB200_DEVICE) != 0));
 }
 
-// tuner.cu: register-tiled polyphase decimating FIR (complex in, real taps), optional fused rotator.
-// Returns 1 if the (M, D) shape is supported and the launch was enqueued, 0 if unsupported, <0 on error.
-PolyTaps* polyphase_prepare(const float* taps, int M, int D, double turns_per_sample, bool phasor_table = false,
+// tuner.cu: register-tiled polyphase decimating FIR with real taps.  polyphase_prepare returns nullptr when no kernel
+// is instantiated for the shape: complex data, for the TunerBlock's fused translator of turns_per_sample if
+// `translator`, or a float32 stream if `real_data`.
+PolyTaps* polyphase_prepare(const float* taps, int M, int D, double turns_per_sample, bool translator = false,
                             bool real_data = false);
 void polyphase_release(PolyTaps* p);
-int launch_polyphase_crcf(const PolyTaps* p, const float2* x, const float2* hist, long long n, float2* y,
-                          long long first, long long n_out, bool rotate, uint64_t turns_fix, uint64_t g0,
-                          cudaStream_t s);
-// real input, real taps, decimating (x / hist / y are float32)
-// z_in != nullptr additionally fuses the output-rate pole z[m] = pole_c z[m-1] + w[m] (state carried in z_in -> z_out)
-int launch_polyphase_rrrf(const PolyTaps* p, const float* x, const float* hist, long long n, float* y,
-                          long long first, long long n_out, cudaStream_t s, float pole_c = 0.f,
-                          const float* z_in = nullptr, float* z_out = nullptr);
+// FirBlock's kernel for taps prepared without a translator: x / hist / y are float2, or float32 for real_data.  A real
+// decimator with pole_in != nullptr additionally fuses the output-rate pole z[m] = pole_c z[m-1] + w[m], its state
+// z[-1] read from pole_in and the last z written to pole_out.  0, or -1 with the error set.
+int launch_polyphase(const PolyTaps* p, const void* x, const void* hist, long long n, void* y, long long first,
+                     long long n_out, cudaStream_t s, float pole_c = 0.f, const float* pole_in = nullptr,
+                     float* pole_out = nullptr);
 bool polyphase_pole_ok(float c);     // the pole's memory fits the kernel's warm-up
 // tuner.cu: fused FrequencyTranslator -> FIR(crcf) -> Downsampler; returns nullptr (with the error set) on failure
 // iqconv.cu: IQFileSource sample format -> ComplexFloat32 (nullptr + error for an unknown format)

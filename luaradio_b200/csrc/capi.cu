@@ -6,6 +6,7 @@
 #include "blocks.h"
 
 #include <cstdarg>
+#include <cstdint>
 #include <cstdio>
 #include <cstring>
 #include <cmath>
@@ -149,10 +150,19 @@ FirBlock::FirBlock(FirKind k, const void* taps_host, unsigned ntaps, unsigned de
 int FirBlock::init() {
     if (d_taps.upload(h_taps.data(), (size_t)M * tap_size) != 0) return -1;
     if (carry(d_hist, (size_t)(M > 1 ? M - 1 : 1) * in_size, cur) != 0) return -1;
-    return fast_init();
+    // register-tiled direct kernel: decimators with <= 128 taps and plain FIRs with <= 32 taps (complex in, real taps)
+    if (kind == FIR_CRCF && !rotate) poly = polyphase_prepare((const float*)h_taps.data(), M, D, 0.0);
+    if (kind == FIR_RRRF && D > 1) poly = polyphase_prepare((const float*)h_taps.data(), M, D, 0.0, false, true);
+    gen_poly = !rotate && D >= 2 && poly_generic_supports(kind, M, D);
+    if (fir_fast_prepare(kind, h_taps.data(), M, D, rotate, rot_fix, &fast) != 0) return -1;
+    if (rotate && !fast) { set_error("fir: fused translator needs the overlap-save path (ntaps <= %d)", FFT_MAX_TAPS); return -1; }
+    return 0;
 }
 
+FirBlock::~FirBlock() { polyphase_release(poly); }
+
 int FirBlock::set_pole(float c) {
+    if (kind != FIR_RRRF || !always_polyphase()) { set_error("fir: the fused output-rate pole needs the real polyphase kernel"); return -1; }
     if (carry(d_pole, sizeof(float), pcur) != 0) return -1;
     has_pole = true;
     pole_c = c;
@@ -175,6 +185,40 @@ long long IirBlock::memory_in() const {
     return w < 0 ? -1 : w + nb;
 }
 
+int FirBlock::set_algorithm(int a) {
+    if (a < LRB200_FIR_AUTO || a > LRB200_FIR_FFT) { set_error("fir: unknown algorithm %d", a); return -1; }
+    algo = a;
+    return 0;
+}
+
+// AUTO: overlap-save once the direct form would be FP32-bound.  float2 FMAs per INPUT sample:
+//   direct = M/D (crcf), 2M/D (cccf), M/2D (rrrf, hilbert);  overlap-save ~ 31 / (L/N) (half for packed real blocks)
+// Direct kernels for these shapes: the generic polyphase kernel where it covers the shape (it beat the
+// overlap-save kernel only for short complex-input real-tap filters, e.g. (D, M) = (2, 16), (3, 33); tap loads from
+// the constant bank pace it), else the catch-all (about 8x off), hence the factors.
+static bool overlap_save_cheaper(const FirBlock& f) {
+    const double per_tap = f.kind == FIR_CCCF ? 2.0 : (f.kind == FIR_CRCF ? 1.0 : (f.gen_poly ? 1.0 : 0.5));
+    const double direct_cost = (f.gen_poly ? 3.0 : 8.0) * per_tap * f.M / f.D;
+    const double fft_cost = f.fast->nparts * 31.0 * FIR_FFT_N / (double)f.fast->block_len() * (f.kind == FIR_RRRF ? 0.5 : 1.0);
+    return direct_cost > fft_cost;
+}
+
+// Which kernel runs a call: tests/fft_fir_ref.py FirModel.plan states the same choices.
+FirPath FirBlock::path(size_t n) const {
+    if (always_polyphase()) return FirPath::Polyphase;
+    // the fused translator exists only in the overlap-save kernel (init refuses a rotating FIR without the plan)
+    const bool fft = rotate || (fast && (algo == LRB200_FIR_FFT || (algo == LRB200_FIR_AUTO && overlap_save_cheaper(*this))));
+    if (!fft) return gen_poly ? FirPath::PolyGeneric : FirPath::Direct;
+    // a forced FFT (or a fused translator) always runs; the automatic choice leaves short calls to the catch-all
+    if (algo != LRB200_FIR_FFT && !rotate && n < 8 * (size_t)fast->block_len()) return FirPath::Direct;
+    return fast->nparts > 1 ? FirPath::DelayLine : FirPath::OverlapSave;
+}
+
+int FirBlock::effective_algorithm() const {
+    const FirPath p = path(SIZE_MAX);
+    return p == FirPath::OverlapSave || p == FirPath::DelayLine ? LRB200_FIR_FFT : LRB200_FIR_DIRECT;
+}
+
 int FirBlock::run(const void* dx, size_t n, void* dy, size_t* n_out, cudaStream_t s) {
     long long first, no;
     decim_plan(consumed, (unsigned)D, n, &first, &no);
@@ -187,10 +231,22 @@ int FirBlock::run(const void* dx, size_t n, void* dy, size_t* n_out, cudaStream_
         if (n >= SIDE_STREAM_MIN) side = side_fork(s);
         if (launch_hist_update(dx, (long long)n, d_hist[cur].get(), d_hist[cur ^ 1].get(), M - 1, (int)in_size, side) != 0) return -1;
     }
-    int rc = fast_run(dx, n, dy, first, no, s);
-    if (rc == 0) rc = launch_fir_generic(kind, dx, d_hist[cur].get(), d_taps.get(), M, D, first, no, dy, s) == 0 ? 1 : -1;
+    const void* hist = d_hist[cur].get();
+    int rc;
+    switch (path(n)) {
+        case FirPath::Polyphase:
+            rc = launch_polyphase(poly, dx, hist, (long long)n, dy, first, no, s, pole_c,
+                                  has_pole ? d_pole[pcur].as<const float>() : nullptr, d_pole[pcur ^ 1].as<float>());
+            break;
+        case FirPath::PolyGeneric:
+            rc = launch_poly_generic(kind, dx, hist, h_taps.data(), M, D, first, (long long)n, no, dy, s);
+            break;
+        case FirPath::OverlapSave: rc = launch_overlap_save(*fast, dx, hist, (long long)n, dy, first, consumed, s); break;
+        case FirPath::DelayLine: rc = launch_delay_line(*fast, dx, hist, (long long)n, dy, s); break;
+        default: rc = launch_fir_generic(kind, dx, hist, d_taps.get(), M, D, first, no, dy, s);     // FirPath::Direct
+    }
     side_join(s, side);
-    if (rc < 0) return -1;
+    if (rc != 0) return -1;
     if (M > 1) cur ^= 1;
     if (has_pole && no > 0) pcur ^= 1;
     consumed += n;

@@ -34,7 +34,7 @@ namespace lrb {
 
 namespace {
 
-constexpr int FF_N = 1024;
+constexpr int FF_N = FIR_FFT_N;
 constexpr int FF_WARPS = 8;                       // warps (= concurrent FFT blocks) per CTA
 constexpr int FF_THREADS = FF_WARPS * 32;
 constexpr int FF_XSTRIDE = 33;                    // padded row stride of the transpose tile (float2 units)
@@ -286,7 +286,7 @@ int launch_fft(const FftArgs& base_args, long long n_int, long long n_edge, cuda
     }
     side_join(s, side);
     LRB_CHECK(cudaGetLastError());
-    return 1;
+    return 0;
 }
 
 // ---------------------------------------------------------------------------------------------
@@ -510,7 +510,7 @@ int launch_fdl_pc(FdlArgs a, cudaStream_t s) {
     }
     side_join(s, side);
     LRB_CHECK(cudaGetLastError());
-    return 1;
+    return 0;
 }
 
 int launch_fdl(const FdlArgs& a, cudaStream_t s) {
@@ -528,34 +528,24 @@ int launch_fdl(const FdlArgs& a, cudaStream_t s) {
 // Host-side plan: tap spectrum (float64 DFT of the zero-extended taps, scaled by 1/N, as
 // firfilter.lua:337-343 does with spectrum_utils.DFT) and the 32x32 inter-pass twiddle table.
 // ---------------------------------------------------------------------------------------------
-struct FirFast {
-    int nparts = 1;            // > 1: uniformly partitioned overlap-save for filters longer than one block allows
-    int part_taps = 0;
-    DeviceBuffer d_H;          // nparts tap spectra, FF_N each
-    DeviceBuffer d_tw;
-    DeviceBuffer d_E;
-    int in_mode = 0;
-};
-
-static constexpr int FFT_MAX_TAPS = 513;       // L >= 512: at most half of every block is overlap
-
-int FirBlock::fast_init() {
-    // register-tiled direct kernel: decimators with <= 128 taps and plain FIRs with <= 32 taps (complex in, real taps)
-    if (kind == FIR_CRCF && !rotate) poly = polyphase_prepare((const float*)h_taps.data(), M, D, 0.0);
-    if (kind == FIR_RRRF && D > 1) poly = polyphase_prepare((const float*)h_taps.data(), M, D, 0.0, false, true);
-    gen_poly = !rotate && D >= 2 && poly_generic_supports(kind, M, D);
+int fir_fast_prepare(FirKind kind, const void* taps, int M, int D, bool rotate, uint64_t rot_fix,
+                     std::unique_ptr<FirFast>* out) {
     if (kind == FIR_HILBERT && D != 1) return 0;
     const bool long_filter = M > FFT_MAX_TAPS;
     // long filters: complex-input, no fused decimation/translator -> P partitions of 512 taps, P passes over x
     if (long_filter && !((kind == FIR_CRCF || kind == FIR_CCCF) && D == 1 && !rotate && M <= 16 * 512)) return 0;
-    fast = new (std::nothrow) FirFast();
+    std::unique_ptr<FirFast> fast(new (std::nothrow) FirFast());
     if (!fast) { set_error("out of memory"); return -1; }
     fast->in_mode = (kind == FIR_RRRF) ? 1 : (kind == FIR_HILBERT ? 2 : 0);
+    fast->M = M;
+    fast->D = D;
     fast->part_taps = long_filter ? 512 : M;
     fast->nparts = long_filter ? (M + 511) / 512 : 1;
+    fast->rotate = rotate;
+    fast->rot_fix = rot_fix;
     const double two_pi = 6.283185307179586476925286766559;
     std::vector<std::complex<double>> h(M);
-    const float* tf = (const float*)h_taps.data();
+    const float* tf = (const float*)taps;
     for (int k = 0; k < M; ++k) {
         if (kind == FIR_CCCF) h[k] = std::complex<double>(tf[2 * k], tf[2 * k + 1]);
         else if (kind == FIR_HILBERT) h[k] = std::complex<double>(k == (M - 1) / 2 ? 1.0 : 0.0, tf[k]);   // delay + j*hilbert (hilberttransform.lua:120-124)
@@ -594,109 +584,57 @@ int FirBlock::fast_init() {
         }
         if (fast->d_E.upload(E.data(), sizeof(float2) * FF_N) != 0) return -1;
     }
+    *out = std::move(fast);
     return 0;
 }
 
-FirBlock::~FirBlock() {
-    polyphase_release(poly);
-    delete fast;
-}
-
-// The algorithm that would run for a long input (what lrb200_fir_get_algorithm reports).
-int FirBlock::effective_algorithm() const {
-    if (rotate) return LRB200_FIR_FFT;                         // the fused translator exists only in the FFT kernel
-    if (!fast || algo == LRB200_FIR_DIRECT) return LRB200_FIR_DIRECT;
-    if (algo == LRB200_FIR_FFT) return LRB200_FIR_FFT;
-    if (poly) return LRB200_FIR_DIRECT;                        // register-tiled polyphase decimator
-    // automatic: overlap-save once the direct form would be FP32-bound.  float2 FMAs per INPUT sample:
-    //   direct = M/D (crcf), 2M/D (cccf), M/2D (rrrf, hilbert);  overlap-save ~ 31 / (L/N) (half for packed real blocks)
-    // Direct kernels for these shapes: the generic polyphase kernel where it covers the shape (it beat the
-    // overlap-save kernel only for short complex-input real-tap filters, e.g. (D, M) = (2, 16), (3, 33); tap loads from
-    // the constant bank pace it), else the catch-all (about 8x off), hence the factors.
-    const double per_tap = kind == FIR_CCCF ? 2.0 : (kind == FIR_CRCF ? 1.0 : (gen_poly ? 1.0 : 0.5));
-    const double direct_cost = (gen_poly ? 3.0 : 8.0) * per_tap * M / D;
-    const int mp = fast->part_taps;
-    const double fft_cost = fast->nparts * 31.0 * FF_N / (double)(FF_N - mp + 1) * (kind == FIR_RRRF ? 0.5 : 1.0);
-    return direct_cost > fft_cost ? LRB200_FIR_FFT : LRB200_FIR_DIRECT;
-}
-
-int FirBlock::set_algorithm(int a) {
-    if (a < LRB200_FIR_AUTO || a > LRB200_FIR_FFT) { set_error("fir: unknown algorithm %d", a); return -1; }
-    algo = a;
+int launch_delay_line(const FirFast& f, const void* x, const void* hist, long long n, void* y, cudaStream_t s) {
+    // hop 512: blocks b cover outputs [512 b, 512 b + 512)
+    const long long nb = (n + FD_HOP - 1) / FD_HOP;
+    for (int p0 = 0; p0 < f.nparts; p0 += FD_MAXPC) {
+        FdlArgs a;
+        a.x = (const float2*)x; a.hist = (const float2*)hist; a.y = (float2*)y;
+        a.H = f.d_H.as<float2>() + (size_t)p0 * FF_N; a.tw = f.d_tw.as<float2>(); a.n = n;
+        a.pc = std::min(FD_MAXPC, f.nparts - p0);
+        a.nblocks = nb;
+        a.b_lo = std::min<long long>(nb, a.pc + p0);          // first block whose ring pre-fill reads x[>= 0]
+        a.b_hi = std::max<long long>(a.b_lo, n / FD_HOP);
+        if (a.b_hi > nb) a.b_hi = nb;
+        a.chunk = 0; a.hist_len = f.M - 1; a.in_shift = p0 * FD_HOP; a.accumulate = p0 > 0 ? 1 : 0;
+        if (launch_fdl(a, s) != 0) return -1;
+    }
     return 0;
 }
 
-int FirBlock::fast_run(const void* dx, size_t n, void* dy, long long first, long long n_out, cudaStream_t s) {
-    if (poly && algo != LRB200_FIR_FFT && kind == FIR_RRRF)
-        return launch_polyphase_rrrf(poly, (const float*)dx, d_hist[cur].as<const float>(), (long long)n, (float*)dy, first, n_out, s,
-                                     pole_c, d_pole[pcur].as<const float>(), d_pole[pcur ^ 1].as<float>());
-    if (has_pole) { set_error("fir: the fused output-rate pole needs the real polyphase kernel"); return -1; }
-    if (poly && algo != LRB200_FIR_FFT)
-        return launch_polyphase_crcf(poly, (const float2*)dx, d_hist[cur].as<const float2>(), (long long)n, (float2*)dy,
-                                     first, n_out, false, 0, consumed, s);
-    const int eff = effective_algorithm();
-    if (gen_poly && eff == LRB200_FIR_DIRECT) {
-        const int rc = launch_poly_generic(kind, dx, d_hist[cur].get(), h_taps.data(), M, D, first, (long long)n, n_out, dy, s);
-        if (rc != 0) return rc;
-    }
-    if (!fast || eff != LRB200_FIR_FFT) {
-        if (rotate) { set_error("fir: fused translator needs the overlap-save path (ntaps <= %d)", FFT_MAX_TAPS); return -1; }
-        return 0;
-    }
-    const int Mp = fast->part_taps;                      // taps convolved per launch (== M unless partitioned)
-    const int L = FF_N - (Mp - 1);
-    // a forced FFT (or a fused translator) always runs; the automatic choice leaves short calls to the direct kernel
-    if (algo != LRB200_FIR_FFT && !rotate && (long long)n < 8LL * L) return 0;
+int launch_overlap_save(const FirFast& f, const void* x, const void* hist, long long n, void* y, long long first,
+                        uint64_t g0, cudaStream_t s) {
+    const int L = f.block_len();
     // blocks of L outputs; in packed-real mode one FFT covers two of them
-    const long long per = (fast->in_mode == 1) ? 2LL * L : (long long)L;
-    const long long nblocks = ((long long)n + per - 1) / per;
-    if (fast->nparts > 1) {
-        // frequency-domain delay line: hop 512, blocks b cover outputs [512 b, 512 b + 512)
-        const long long nb = ((long long)n + FD_HOP - 1) / FD_HOP;
-        for (int p0 = 0; p0 < fast->nparts; p0 += FD_MAXPC) {
-            FdlArgs a;
-            a.x = (const float2*)dx; a.hist = d_hist[cur].as<const float2>(); a.y = (float2*)dy;
-            a.H = fast->d_H.as<float2>() + (size_t)p0 * FF_N; a.tw = fast->d_tw.as<float2>(); a.n = (long long)n;
-            a.pc = std::min(FD_MAXPC, fast->nparts - p0);
-            a.nblocks = nb;
-            a.b_lo = std::min<long long>(nb, a.pc + p0);          // first block whose ring pre-fill reads x[>= 0]
-            a.b_hi = std::max<long long>(a.b_lo, (long long)n / FD_HOP);
-            if (a.b_hi > nb) a.b_hi = nb;
-            a.chunk = 0; a.hist_len = M - 1; a.in_shift = p0 * FD_HOP; a.accumulate = p0 > 0 ? 1 : 0;
-            if (launch_fdl(a, s) < 0) return -1;
-        }
-        return 1;
+    const long long per = (f.in_mode == 1) ? 2LL * L : (long long)L;
+    const long long nblocks = (n + per - 1) / per;
+    // interior blocks [b_lo, b_hi): b*per - (M-1) >= 0  and  (b+1)*per <= n
+    long long b_lo = ((long long)(f.M - 1) + per - 1) / per;
+    if (b_lo < 1) b_lo = 1;
+    long long b_hi = n / per;
+    if (b_hi > nblocks) b_hi = nblocks;
+    if (b_hi < b_lo) b_hi = b_lo;
+    if (b_lo > nblocks) { b_lo = nblocks; b_hi = nblocks; }
+    FftArgs a;
+    a.x = x; a.hist = hist; a.y = y; a.H = f.d_H.as<float2>(); a.tw = f.d_tw.as<float2>(); a.E = f.d_E.as<float2>();
+    a.n = n; a.b_lo = b_lo; a.b_hi = b_hi; a.nwork = 0; a.first = first;
+    a.turns_fix = f.rot_fix; a.g0 = g0; a.M = f.M; a.D = f.D;
+    // edge work list: blocks [0, b_lo) and [b_hi, nblocks); the kernel maps e -> (e < b_lo ? e : b_hi + e - b_lo)
+    const long long n_int = b_hi - b_lo, n_edge = b_lo + (nblocks - b_hi);
+    const bool dec = f.D > 1;
+    switch (f.in_mode) {
+        case 0:
+            if (f.rotate) return launch_fft<0, true, true>(a, n_int, n_edge, s);   // fused translator always uses the DEC store (D may be 1)
+            return dec ? launch_fft<0, false, true>(a, n_int, n_edge, s) : launch_fft<0, false, false>(a, n_int, n_edge, s);
+        case 1:
+            return dec ? launch_fft<1, false, true>(a, n_int, n_edge, s) : launch_fft<1, false, false>(a, n_int, n_edge, s);
+        default:
+            return launch_fft<2, false, false>(a, n_int, n_edge, s);
     }
-    {
-        // interior blocks [b_lo, b_hi): b*per - (M-1) >= 0  and  (b+1)*per <= n
-        long long b_lo = ((long long)(Mp - 1) + per - 1) / per;
-        if (b_lo < 1) b_lo = 1;
-        long long b_hi = (long long)n / per;
-        if (b_hi > nblocks) b_hi = nblocks;
-        if (b_hi < b_lo) b_hi = b_lo;
-        if (b_lo > nblocks) { b_lo = nblocks; b_hi = nblocks; }
-        FftArgs a;
-        a.x = dx; a.hist = d_hist[cur].get(); a.y = dy; a.H = fast->d_H.as<float2>(); a.tw = fast->d_tw.as<float2>(); a.E = fast->d_E.as<float2>();
-        a.n = (long long)n; a.b_lo = b_lo; a.b_hi = b_hi; a.nwork = 0; a.first = first;
-        a.turns_fix = rot_fix; a.g0 = consumed; a.M = Mp; a.D = D;
-        // edge work list: blocks [0, b_lo) and [b_hi, nblocks); the kernel maps e -> (e < b_lo ? e : b_hi + e - b_lo)
-        const long long n_int = b_hi - b_lo, n_edge = b_lo + (nblocks - b_hi);
-        const bool dec = D > 1;
-        int rc;
-        switch (fast->in_mode) {
-            case 0:
-                if (rotate) rc = launch_fft<0, true, true>(a, n_int, n_edge, s);   // fused translator always uses the DEC store (D may be 1)
-                else rc = dec ? launch_fft<0, false, true>(a, n_int, n_edge, s) : launch_fft<0, false, false>(a, n_int, n_edge, s);
-                break;
-            case 1:
-                rc = dec ? launch_fft<1, false, true>(a, n_int, n_edge, s) : launch_fft<1, false, false>(a, n_int, n_edge, s);
-                break;
-            default:
-                rc = launch_fft<2, false, false>(a, n_int, n_edge, s);
-        }
-        if (rc < 0) return -1;
-    }
-    return 1;
 }
 
 }  // namespace lrb

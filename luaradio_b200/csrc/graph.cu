@@ -116,10 +116,11 @@ static int fuse_noble_identity(const Blocks& blocks, size_t i, Rewrite* out) {
     }
     auto nf = make_block<FirBlock>(FIR_RRRF, hc.data(), (unsigned)Mc, (unsigned)Dd, true);
     if (!nf) return -1;
+    // only worth it when the polyphase kernel has this shape (at AUTO, the block runs it whenever it has it)
+    if (!nf->always_polyphase()) return 0;
     nf->set_algorithm(fir->algo);
-    if (!nf->poly) return 0;         // only worth it when the polyphase kernel has this shape
     nf->name = "fir*iir1_rrrf(" + std::to_string(Mc) + ",/" + std::to_string(Dd) + ")";
-    if (nf->algo != LRB200_FIR_FFT && polyphase_pole_ok((float)cp)) {
+    if (nf->always_polyphase() && polyphase_pole_ok((float)cp)) {
         // the pole's memory (|c^D|^64 <= 1e-8) fits the kernel's own warm-up: ONE stage
         if (nf->set_pole((float)cp) != 0) return -1;
         nf->name += "+pole";

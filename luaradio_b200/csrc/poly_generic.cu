@@ -128,17 +128,13 @@ int launch_pg(const GenParams& P, const void* x, const void* hist, void* y, cuda
     k<<<(unsigned)tiles, PG_THREADS, smem, s>>>((const T*)x, (const T*)hist, (T*)y, P);
     count_launch();
     LRB_CHECK(cudaGetLastError());
-    return 1;
+    return 0;
 }
 
 template <int D>
 int launch_pg_d(FirKind kind, const GenParams& P, const void* x, const void* hist, void* y, cudaStream_t s) {
-    switch (kind) {
-        case FIR_CRCF: return launch_pg<float2, D, false>(P, x, hist, y, s);
-        case FIR_CCCF: return launch_pg<float2, D, true>(P, x, hist, y, s);
-        case FIR_RRRF: return launch_pg<float, D, false>(P, x, hist, y, s);
-        default: return 0;
-    }
+    if (kind == FIR_RRRF) return launch_pg<float, D, false>(P, x, hist, y, s);
+    return kind == FIR_CCCF ? launch_pg<float2, D, true>(P, x, hist, y, s) : launch_pg<float2, D, false>(P, x, hist, y, s);
 }
 
 }  // namespace
@@ -155,12 +151,10 @@ bool poly_generic_supports(FirKind kind, int M, int D) {
     return (size_t)(PG_TO + Qn + PG_TO / PG_R + 4) * D * elem <= (size_t)200 * 1024;
 }
 
-// taps: natural order (float, or interleaved complex for FIR_CCCF).  Returns 1 if launched, 0 if the shape is not
-// covered, < 0 on error.
+// taps: natural order (float, or interleaved complex for FIR_CCCF); (kind, M, D) covered.  0, or -1 with the error set.
 int launch_poly_generic(FirKind kind, const void* x, const void* hist, const void* taps_host, int M, int D,
                         long long first, long long n, long long n_out, void* y, cudaStream_t s) {
-    if (!poly_generic_supports(kind, M, D)) return 0;
-    if (n_out <= 0) return 1;
+    if (n_out <= 0) return 0;
     GenParams P;
     std::memset(&P, 0, sizeof(P));
     const int Qn = (M + D - 1) / D, z = Qn * D - M;
@@ -185,7 +179,8 @@ int launch_poly_generic(FirKind kind, const void* x, const void* hist, const voi
         case 20: return launch_pg_d<20>(kind, P, x, hist, y, s);
         case 25: return launch_pg_d<25>(kind, P, x, hist, y, s);
     }
-    return 0;
+    set_error("fir: no generic polyphase kernel for D = %d", D);
+    return -1;
 }
 
 }  // namespace lrb

@@ -738,12 +738,15 @@ int encode_tile_map(CUtensorMap* map, const float2* base, long long rows, int rd
     return 0;
 }
 
+// prev_in / prev_out / inv_gain are the kernel's: the discriminator's previous tuner output and 1 / gain (DISC), or the
+// pole's float32 state (POLE, its coefficient is in P).  0, or -1 with the error set.
 template <int D, int Q, bool ROT, bool DISC, bool REAL = false, bool POLE = false>
 int launch_shape(PolyParams P, const float* hr_base, const float2* x, const float2* hist, long long n,
                  void* y, long long first, long long n_out, const float2* prev_in, float2* prev_out, float inv_gain,
                  cudaStream_t s) {
     using S = PolyShape<D, Q>;
     static_assert(S::T <= PT_MAXTAPS, "taps table too small");
+    static_assert(S::ITERS <= PT_MAXIT, "step table too short");
     // function attributes are per device: a process that drives several GPUs configures each once
     static bool configured_dev[LRB_MAX_DEVICES] = {false};
     static int ctas_dev[LRB_MAX_DEVICES] = {0};
@@ -824,7 +827,7 @@ int launch_shape(PolyParams P, const float* hr_base, const float2* x, const floa
     }
     side_join(s, side);
     LRB_CHECK(cudaGetLastError());
-    return 1;
+    return 0;
 }
 
 }  // namespace
@@ -834,18 +837,17 @@ struct PolyTaps {
     float hr[PT_MAXTAPS];        // reversed taps, Q*D entries: hr[i'] = h[Q*D-1-i']
     uint64_t turns_fix;
     float2 step[PT_MAXIT];       // per-staging-iteration phasor advance (see PolyParams)
-    bool rotates = false;        // a translator is fused
     bool real_data = false;      // float32 stream (REAL kernel variant)
 };
 
-static int shape_q(int M, int D, bool rotates) {
+static int shape_q(int M, int D, bool translator) {
     // Instantiated shapes.  Each one is a handful of fully unrolled ~2500-instruction kernels (minutes of ptxas
     // time), so the list is exactly what the reference's own graphs produce on the hot path:
     //   (D, Q) = (5, 26): TunerBlock / DecimatorBlock with the default 128 taps and decimation 5
     //            (examples/rtlsdr_wbfm_mono.lua), with or without the translator / discriminator;
     //   (1, 16), (1, 32): plain FIRs with up to 16 / 32 real taps (below the overlap-save break-even).
     // Every other decimating or translating FIR runs the overlap-save kernel (fir_fft.cu), which fuses both.
-    if (D == 1 && !rotates) return M <= 16 ? 16 : (M <= 32 ? 32 : 0);
+    if (D == 1 && !translator) return M <= 16 ? 16 : (M <= 32 ? 32 : 0);
     if (D == 5 && M > 65 && M <= 128) return 26;
     return 0;
 }
@@ -857,8 +859,8 @@ static int shape_q_real(int M, int D) {
     return 0;
 }
 
-PolyTaps* polyphase_prepare(const float* taps, int M, int D, double turns_per_sample, bool phasor_table, bool real_data) {
-    int Q = real_data ? shape_q_real(M, D) : shape_q(M, D, phasor_table);
+PolyTaps* polyphase_prepare(const float* taps, int M, int D, double turns_per_sample, bool translator, bool real_data) {
+    int Q = real_data ? shape_q_real(M, D) : shape_q(M, D, translator);
     if (!Q) return nullptr;
     PolyTaps* p = new (std::nothrow) PolyTaps();
     if (!p) return nullptr;
@@ -870,7 +872,6 @@ PolyTaps* polyphase_prepare(const float* taps, int M, int D, double turns_per_sa
         p->hr[i] = (i < Q * D && k < M) ? taps[k] : 0.0f;
     }
     p->turns_fix = turns_to_fix(turns_per_sample);
-    p->rotates = phasor_table;
     {
         // step[it] = exp(j 2 pi turns * 2*PT_THREADS*it) from the SAME fixed-point turns the kernel uses
         const double two_pi = 6.283185307179586476925286766559;
@@ -886,69 +887,39 @@ PolyTaps* polyphase_prepare(const float* taps, int M, int D, double turns_per_sa
 
 void polyphase_release(PolyTaps* p) { delete p; }
 
-#define LRB_SHAPE_FULL(DD, QQ)                                                                                         \
-    if (p->D == DD && p->Q == QQ) {                                                                                    \
-        static_assert(PolyShape<DD, QQ>::ITERS <= PT_MAXIT, "step table too short");                                   \
-        if (disc) return launch_shape<DD, QQ, true, true>(P, p->hr, x, hist, n, y, first, n_out, prev_in, prev_out, inv_gain, s); \
-        return rot ? launch_shape<DD, QQ, true, false>(P, p->hr, x, hist, n, y, first, n_out, nullptr, nullptr, 0.f, s)    \
-                   : launch_shape<DD, QQ, false, false>(P, p->hr, x, hist, n, y, first, n_out, nullptr, nullptr, 0.f, s);  \
-    }
-#define LRB_SHAPE_PLAIN(DD, QQ)                                                                                        \
-    if (p->D == DD && p->Q == QQ && !rot && !disc) {                                                                   \
-        static_assert(PolyShape<DD, QQ>::ITERS <= PT_MAXIT, "step table too short");                                   \
-        return launch_shape<DD, QQ, false, false>(P, p->hr, x, hist, n, y, first, n_out, nullptr, nullptr, 0.f, s); \
-    }
+bool polyphase_pole_ok(float c) { return std::pow(std::fabs((double)c), (double)PT_POLE_WARM) <= 1e-8; }
 
-static int launch_polyphase_any(const PolyTaps* p, const float2* x, const float2* hist, long long n, void* y,
-                                long long first, long long n_out, bool rotate, bool disc, uint64_t g0,
-                                const float2* prev_in, float2* prev_out, float inv_gain, cudaStream_t s) {
-    if (!p) return 0;
-    if (n_out <= 0) return 1;
-    const bool rot = rotate && p->rotates;
-    if (disc && !rot) {
-        // the fused discriminator is instantiated together with the translator; a zero offset gets the all-ones table
-        set_error("tuner: discriminator fusion needs the translator path");
-        return -1;
-    }
+// the parameters every launch for p starts from; g0 is the global index of x[0] (read with the translator only)
+static PolyParams poly_params(const PolyTaps* p, uint64_t g0) {
     PolyParams P;
     std::memset(&P, 0, sizeof(P));
     P.turns_fix = p->turns_fix;
     std::memcpy(P.step, p->step, sizeof(P.step));
     P.g0 = g0;
     P.M = p->M;
-    if (p->real_data) {
-        if (rot || disc) { set_error("polyphase: the real-stream kernel has no translator / discriminator"); return -1; }
-        const bool pole = prev_in != nullptr;
-        if (pole) {
-            // inv_gain carries the pole c; prev_in / prev_out its carried state (float32)
-            const double c = (double)inv_gain;
-            P.pole_c = inv_gain;
-            double pw = std::pow(c, (double)PT_R);
-            for (int k = 0; k < 6; ++k) { P.pole_cp[k] = (float)pw; pw = pw * pw; }
-        }
-        if (p->D == 5 && p->Q == 27)
-            return pole ? launch_shape<5, 27, false, false, true, true>(P, p->hr, x, hist, n, y, first, n_out, prev_in, prev_out, 0.f, s)
-                        : launch_shape<5, 27, false, false, true, false>(P, p->hr, x, hist, n, y, first, n_out, nullptr, nullptr, 0.f, s);
-        return 0;
+    return P;
+}
+
+int launch_polyphase(const PolyTaps* p, const void* x, const void* hist, long long n, void* y, long long first,
+                     long long n_out, cudaStream_t s, float pole_c, const float* pole_in, float* pole_out) {
+    if (n_out <= 0) return 0;
+    PolyParams P = poly_params(p, 0);
+    // the kernel takes every stream as float2; the real variant (Q = 27) reads float32 samples through these pointers
+    const float2* xs = (const float2*)x;
+    const float2* hs = (const float2*)hist;
+    if (p->D == 5 && p->Q == 27 && pole_in) {
+        P.pole_c = pole_c;
+        double pw = std::pow((double)pole_c, (double)PT_R);
+        for (int k = 0; k < 6; ++k) { P.pole_cp[k] = (float)pw; pw = pw * pw; }
+        return launch_shape<5, 27, false, false, true, true>(P, p->hr, xs, hs, n, y, first, n_out, (const float2*)pole_in,
+                                                             (float2*)pole_out, 0.f, s);
     }
-    LRB_SHAPE_PLAIN(1, 16) LRB_SHAPE_PLAIN(1, 32)
-    LRB_SHAPE_FULL(5, 26)
-    return 0;
-}
-
-bool polyphase_pole_ok(float c) { return std::pow(std::fabs((double)c), (double)PT_POLE_WARM) <= 1e-8; }
-
-int launch_polyphase_rrrf(const PolyTaps* p, const float* x, const float* hist, long long n, float* y,
-                          long long first, long long n_out, cudaStream_t s, float pole_c, const float* z_in, float* z_out) {
-    return launch_polyphase_any(p, (const float2*)x, (const float2*)hist, n, y, first, n_out, false, false, 0,
-                                (const float2*)z_in, (float2*)z_out, pole_c, s);
-}
-
-int launch_polyphase_crcf(const PolyTaps* p, const float2* x, const float2* hist, long long n, float2* y,
-                          long long first, long long n_out, bool rotate, uint64_t turns_fix, uint64_t g0,
-                          cudaStream_t s) {
-    (void)turns_fix;
-    return launch_polyphase_any(p, x, hist, n, y, first, n_out, rotate, false, g0, nullptr, nullptr, 0.f, s);
+    if (p->D == 5 && p->Q == 27) return launch_shape<5, 27, false, false, true, false>(P, p->hr, xs, hs, n, y, first, n_out, nullptr, nullptr, 0.f, s);
+    if (p->D == 1 && p->Q == 16) return launch_shape<1, 16, false, false>(P, p->hr, xs, hs, n, y, first, n_out, nullptr, nullptr, 0.f, s);
+    if (p->D == 1 && p->Q == 32) return launch_shape<1, 32, false, false>(P, p->hr, xs, hs, n, y, first, n_out, nullptr, nullptr, 0.f, s);
+    if (p->D == 5 && p->Q == 26) return launch_shape<5, 26, false, false>(P, p->hr, xs, hs, n, y, first, n_out, nullptr, nullptr, 0.f, s);
+    set_error("polyphase: no kernel for (D, Q) = (%d, %d)", p->D, p->Q);
+    return -1;
 }
 
 // ---------------------------------------------------------------------------------------------
@@ -991,11 +962,17 @@ struct TunerBlock : Block {
             if (n >= SIDE_STREAM_MIN) side = side_fork(s);
             if (launch_hist_update(dx, (long long)n, d_hist[cur].get(), d_hist[cur ^ 1].get(), M - 1, 8, side) != 0) return -1;
         }
-        int rc = launch_polyphase_any(pt.get(), (const float2*)dx, d_hist[cur].as<const float2>(), (long long)n, dy, first, no, true,
-                                      disc, consumed, d_prev[pcur].as<const float2>(), d_prev[pcur ^ 1].as<float2>(),
-                                      disc ? 1.0f / gain : 0.f, s);
+        int rc = 0;
+        if (no > 0) {
+            const PolyParams P = poly_params(pt.get(), consumed);
+            const float2* x = (const float2*)dx;
+            const float2* h = d_hist[cur].as<const float2>();
+            rc = disc ? launch_shape<5, 26, true, true>(P, pt->hr, x, h, (long long)n, dy, first, no, d_prev[pcur].as<const float2>(),
+                                                        d_prev[pcur ^ 1].as<float2>(), 1.0f / gain, s)
+                      : launch_shape<5, 26, true, false>(P, pt->hr, x, h, (long long)n, dy, first, no, nullptr, nullptr, 0.f, s);
+        }
         side_join(s, side);
-        if (rc <= 0) { if (rc == 0) set_error("tuner: unsupported shape"); return -1; }
+        if (rc != 0) return -1;
         if (disc && no > 0) pcur ^= 1;
         if (M > 1) cur ^= 1;
         consumed += n;
@@ -1005,7 +982,8 @@ struct TunerBlock : Block {
 
 std::unique_ptr<Block> make_tuner(double turns_per_sample, const float* taps, int ntaps, int decim, float disc_gain) {
     std::unique_ptr<PolyTaps> p(polyphase_prepare(taps, ntaps, decim, turns_per_sample, true));
-    if (!p) return nullptr;      // unsupported shape: the graph keeps the blocks separate
+    // unsupported shape: the graph keeps the blocks separate (shape_q has one translating shape, which run() launches)
+    if (!p || p->D != 5 || p->Q != 26) return nullptr;
     return make_block<TunerBlock>(std::move(p), disc_gain);
 }
 

@@ -2,7 +2,7 @@
 overlap-save FIR kernels (fir_fft.cu: fir_fft1024_kernel, fir_fft_fdl_kernel) and the direct kernels that take over
 from them (fir_direct.cu fir_generic_kernel, poly_generic.cu).
 
-Geometry.  `FirModel` makes the choices FirBlock::run / fast_run / launch_fft / launch_fdl_pc make, call by call: which
+Geometry.  `FirModel` makes the choices FirBlock::path / launch_fft / launch_fdl_pc make, call by call: which
 path runs, the blocks it cuts and how many kernels it launches (1 for the history update when M > 1, then per
 (partition group) launch +1 for edge work and +1 for interior blocks, or +1 for a direct kernel that has outputs).  A
 graph in device mode launches nothing of its own (graph.cu run_device only calls the stages), so the per-call count
