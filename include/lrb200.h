@@ -167,7 +167,9 @@ lrb200_downsample_t* lrb200_downsample_create(unsigned factor, unsigned elem_siz
  * (:113-179): y[n] = (sum_j b[j] x[n-j] - sum_{j>=1} a[j] y[n-j]) / a[0], zero initial state.
  * Single pole (na <= 2): block-parallel affine scan (decoupled look-back, or a warm-up restart when the pole's
  * memory is shorter than 512 samples).  Higher orders (na, nb <= 10): direct form I in time-parallel chunks
- * with a warm-up measured from the filter's impulse response; short calls are the plain sequential recurrence. */
+ * with a warm-up measured from the filter's impulse response; short calls are the plain sequential recurrence.
+ * Longer filters (nb or na in 11..64): state-space scan in double with a decoupled look-back, exact up to rounding for
+ * any pole radius.  More than 64 taps on either side, or a[0] == 0, is refused. */
 typedef lrb200_block_t lrb200_iir_t;
 lrb200_iir_t* lrb200_iir_create_rrrf(const float32_t* b, unsigned nb, const float32_t* a, unsigned na, unsigned flags);
 lrb200_iir_t* lrb200_iir_create_crcf(const float32_t* b, unsigned nb, const float32_t* a, unsigned na, unsigned flags);

@@ -212,6 +212,29 @@ struct IirGeneralBlock : Block {
     long long memory_in() const override { return warm < 0 ? -1 : warm + nb; }
 };
 
+// iir_order.cu: IIRFilterBlock with more than 10 taps on either side (up to 64 each): a state-space scan in double with a
+// decoupled look-back over 2048-sample tiles, exact for any pole radius
+constexpr int IIR_ORDER_MAX_TAPS = 64;
+constexpr int IIR_ORDER_MAX_TILES = 1 << 17;        // 2048-sample tiles per launch (256 Mi samples)
+struct IirOrderBlock : Block {
+    bool complex_data = false;
+    int nb = 1, q = 0;                                // feed-forward taps, feedback order na - 1
+    std::vector<double> b, cdiv;                      // b[j] / a0;  cdiv[j] = -a[j] / a0 (j >= 1)
+    long long decay = -1;                             // samples until the impulse response of 1/A(z) is below 1e-10 of its peak
+    DeviceBuffer d_xhist[2];                          // last nb - 1 inputs (exact in the input type), oldest first
+    DeviceBuffer d_ystate[2];                         // last q outputs in double, most recent first
+    int cur = 0;
+    DeviceBuffer d_mats, d_hom;                       // M^V, M^(T e) for e < look-back window; homogeneous response table
+    // look-back scratch, not state (as LevelBlock): tickets count up from ticket_base, records are tagged with epoch
+    DeviceBuffer d_ticket, d_flags, d_agg, d_pfx;
+    unsigned long long ticket_base = 0;
+    unsigned epoch = 0;
+    IirOrderBlock(bool cplx, const float* b, unsigned nb, const float* a, unsigned na, bool dev);
+    int init() override;
+    int run(const void* dx, size_t n, void* dy, size_t* n_out, cudaStream_t s) override;
+    long long memory_in() const override { return decay; }
+};
+
 struct C2fBlock : Block {
     int op = 0;                       // 0 = magnitude, 1 = real part
     C2fBlock(int op, bool dev);

@@ -609,8 +609,13 @@ lrb200_downsample_t* lrb200_downsample_create(unsigned factor, unsigned elem_siz
 static lrb200_block_t* iir_create(bool cplx, const float32_t* b, unsigned nb, const float32_t* a, unsigned na, unsigned flags) {
     if (ensure_init() != 0) return nullptr;
     if (!b || nb == 0 || !a || na == 0) { set_error("iir: b and a taps must be non-empty"); return nullptr; }
-    if (nb > 10 || na > 10) { set_error("iir: at most 10 feed-forward and 10 feedback taps"); return nullptr; }
+    if (nb > IIR_ORDER_MAX_TAPS || na > IIR_ORDER_MAX_TAPS) {
+        set_error("iir: at most %d feed-forward and %d feedback taps", IIR_ORDER_MAX_TAPS, IIR_ORDER_MAX_TAPS);
+        return nullptr;
+    }
     if (a[0].value == 0.0f) { set_error("iir: a[0] must be non-zero"); return nullptr; }
+    if (nb > 10 || na > 10)
+        return create_block<IirOrderBlock>(flags, cplx, (const float*)b, nb, (const float*)a, na);
     if (na > 2 || nb > 9)
         return create_block<IirGeneralBlock>(flags, cplx, (const float*)b, nb, (const float*)a, na);
     return create_block<IirBlock>(flags, cplx, (const float*)b, nb, (const float*)a, na);
