@@ -606,6 +606,17 @@ lrb200_downsample_t* lrb200_downsample_create(unsigned factor, unsigned elem_siz
     return create_block<DownsampleBlock>(flags, factor, elem_size);
 }
 
+// IirBlock and IirGeneralBlock run fl32(b / a0) and fl32(a / a0).  Unless every quotient is exact (a0 = +-2^k, or taps
+// that happen to divide), that is a different filter from the reference's, which divides by a0 in double: near the unit
+// circle one rounding of c = -a1 / a0 moves the gain by about u32 / (1 - |c|), 1e-3 for a 10 Hz pole at 1 MHz.  Such
+// filters go to IirOrderBlock, which keeps b / a0 and a / a0 in double.
+static bool normalisation_exact(const float32_t* b, unsigned nb, const float32_t* a, unsigned na) {
+    const double a0 = a[0].value;
+    for (unsigned j = 0; j < nb; ++j) if ((double)(float)(b[j].value / a0) != b[j].value / a0) return false;
+    for (unsigned j = 0; j < na; ++j) if ((double)(float)(a[j].value / a0) != a[j].value / a0) return false;
+    return true;
+}
+
 static lrb200_block_t* iir_create(bool cplx, const float32_t* b, unsigned nb, const float32_t* a, unsigned na, unsigned flags) {
     if (ensure_init() != 0) return nullptr;
     if (!b || nb == 0 || !a || na == 0) { set_error("iir: b and a taps must be non-empty"); return nullptr; }
@@ -614,7 +625,7 @@ static lrb200_block_t* iir_create(bool cplx, const float32_t* b, unsigned nb, co
         return nullptr;
     }
     if (a[0].value == 0.0f) { set_error("iir: a[0] must be non-zero"); return nullptr; }
-    if (nb > 10 || na > 10)
+    if (nb > 10 || na > 10 || !normalisation_exact(b, nb, a, na))
         return create_block<IirOrderBlock>(flags, cplx, (const float*)b, nb, (const float*)a, na);
     if (na > 2 || nb > 9)
         return create_block<IirGeneralBlock>(flags, cplx, (const float*)b, nb, (const float*)a, na);

@@ -203,6 +203,19 @@ def _causal_conv(h, w):
     return np.maximum(r, 0.0) * (1 + 1e-9) + 1e-12 * float(np.max(r))
 
 
+def ref_error(bn, cn, x, ref, cplx, through):
+    """E_ref in units of u64: the float64 reference's own rounding.  Per sample the products of bn with L inputs and of
+    cn with L outputs (L the longer side), (nb + q + 3) times the largest such magnitude sum within L either side, taken
+    through the filter's |h| by `through`."""
+    N = len(x)
+    L = max(len(bn), len(cn) + 1)
+    tm = np.convolve(mag(np.asarray(x).astype(np.complex128 if cplx else np.float64)), np.abs(bn))[:N]
+    if len(cn):
+        tm += np.convolve(mag(np.concatenate([[0.0], ref[:-1]])), np.abs(cn))[:N]
+    tw = scipy.ndimage.maximum_filter1d(tm, 2 * L - 1) if N else tm      # terms of the samples within L either side
+    return through((len(bn) + len(cn) + 3) * tw)
+
+
 def bound(b, a, xs, cplx):
     """(model outputs, float64 reference, per-output bound) of the stream of calls xs (see the module docstring)"""
     m = OrderModel(b, a, cplx)
@@ -217,13 +230,7 @@ def bound(b, a, xs, cplx):
     N = len(x)
     bn, cn = _norm(b, a)
     h = impulse(cn, N)
-    # the reference's own rounding: per sample the products of b with L inputs and of a with L outputs, L the longer side
-    L = max(len(bn), len(cn) + 1)
-    tm = np.convolve(mag(x.astype(np.complex128 if cplx else np.float64)), np.abs(bn))[:N]
-    if len(cn):
-        tm += np.convolve(mag(np.concatenate([[0.0], ref[:-1]])), np.abs(cn))[:N]
-    tw = scipy.ndimage.maximum_filter1d(tm, 2 * L - 1) if N else tm      # terms of the samples within L either side
-    e_ref = _causal_conv(h, (len(bn) + len(cn) + 3) * tw)
+    e_ref = ref_error(bn, cn, x, ref, cplx, lambda w: _causal_conv(h, w))
     e_alg = _causal_conv(h, inj) + direct
     bnd = 2 * U32 * np.abs(ref) + C_BOUND * U64 * (e_alg + e_ref)
     return y, ref, bnd

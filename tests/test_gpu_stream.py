@@ -13,6 +13,7 @@ import luaradio_b200 as radio
 from luaradio_b200 import _lib
 from luaradio_b200.types import ComplexFloat32, Float32, Vector
 from oracle import lr_oracle as O
+from tests import iir_small_ref as S
 
 pytestmark = pytest.mark.gpu
 
@@ -139,9 +140,12 @@ def test_single_pole_iir_long_stream(cplx):
         (radio.SinglepoleHighpassFilterBlock, [1e3], 48e3, O.singlepole_highpass_taps(1e3, 48e3)),
     ):
         blk = mk(cls, args, t, rate)
-        got = stream(blk, x, ragged(rng, n, 0, 90000))
-        ref = O.IIRFilterFast(taps[0], taps[1], cplx).process(x)
-        close(got, ref)
+        cuts = ragged(rng, n, 0, 90000)
+        got = stream(blk, x, cuts)
+        # the per-output bound of tests/iir_small_ref.py, over the same calls
+        _, ref, bnd, _ = S.scan_bound(taps[0], taps[1], [x[a:b] for a, b in cuts], cplx)
+        assert S.excess(got, ref, bnd) <= 1.0
+        close(got, O.IIRFilterFast(taps[0], taps[1], cplx).process(x))
         blk.cleanup()
 
 
@@ -301,10 +305,15 @@ def test_general_iir_long_stream(cplx):
     for order, wn in ((2, 0.3), (4, 0.2), (8, 0.45)):
         b, a = scipy.signal.butter(order, wn)
         b, a = b.astype(np.float32), a.astype(np.float32)
-        ref = O.IIRFilterFast(b, a, cplx).process(x)
+        ref32 = O.IIRFilterFast(b, a, cplx).process(x)
         for cuts in ([(0, n)], ragged(rng, n, 0, 70000)):
             blk = mk(radio.IIRFilterBlock, [Float32.vector_from_array(b), Float32.vector_from_array(a)], t)
-            close(stream(blk, x, cuts), ref)
+            got = stream(blk, x, cuts)
+            # the per-output bound of tests/iir_small_ref.py over the same calls, and the 1e-5 tolerance, which is
+            # tighter than the bound for butter(4, 0.2) and butter(8, 0.45) (their direct form amplifies rounding)
+            ref, bnd, _ = S.general_bound(b, a, [x[lo:hi] for lo, hi in cuts], cplx)
+            assert S.excess(got, ref, bnd) <= 1.0
+            close(got, ref32)
             blk.cleanup()
 
 
