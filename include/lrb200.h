@@ -317,14 +317,27 @@ void   lrb200_graph_destroy(lrb200_graph_t* g);
  * owned by the DAG afterwards.  An input / output reference is  node_id * 4 + output_port,  or -1 for the DAG's single
  * input.  All inputs of a node must deliver the same number of samples per call (converging paths with equal rate
  * changes; the reference's PipeMux, radio/core/pipe.lua:495-615, would buffer a surplus).  lrb200_dag_execute: HOST in,
- * HOST outs -- one upload, the node launches in order, one download per output, one synchronize. */
+ * HOST outs -- one upload, the node launches in order, one download per output, one synchronize.
+ * lrb200_dag_execute_device: the same launches on DEVICE pointers, asynchronous on the library stream with no synchronize
+ * (the output counts are host arithmetic): reads no byte outside [dx, dx + n samples), writes no byte outside each
+ * [dy[k], dy[k] + n_out[k] samples), natural alignment only (as LRB200_DEVICE above).  Refused in super-chunk mode.
+ * lrb200_dag_set_superchunk / lrb200_dag_flush: super-chunk mode with the semantics of lrb200_graph_set_superchunk /
+ * _flush, every output port with its own pinned slots; execute returns, for every port, the outputs of the slots completed
+ * earlier (possibly zero), all ports' counts from the same slots.  Set the outputs first.  Changing the size with a slot
+ * pending is an error (flush first), and so is a flush with no execute since the mode was set, the last flush or reset.
+ * lrb200_dag_max_output is the room `y[output]` of the next execute(n) (or flush, n = 0) must have, in either mode.
+ * lrb200_dag_reset waits for the slots in flight and drops them with the partial slot (the super-chunk size stays), then
+ * zeroes every node's state: the DAG then computes what a fresh one does. */
 typedef struct lrb200_dag_s lrb200_dag_t;
 lrb200_dag_t* lrb200_dag_create(void);
 int    lrb200_dag_add_block(lrb200_dag_t* d, lrb200_block_t* q, const int* inputs, unsigned num_inputs);   /* node id or -1 */
 int    lrb200_dag_add_graph(lrb200_dag_t* d, lrb200_graph_t* g, int input);                                /* node id or -1 */
 int    lrb200_dag_set_outputs(lrb200_dag_t* d, const int* outputs, unsigned num_outputs);
 int    lrb200_dag_execute(lrb200_dag_t* d, const void* x, size_t n, void* const* y, size_t* n_out);        /* n_out[k] per output */
+int    lrb200_dag_execute_device(lrb200_dag_t* d, const void* dx, size_t n, void* const* dy, size_t* n_out); /* DEVICE in/outs, async */
 size_t lrb200_dag_max_output(const lrb200_dag_t* d, unsigned output, size_t n);
+int    lrb200_dag_set_superchunk(lrb200_dag_t* d, size_t samples);
+int    lrb200_dag_flush(lrb200_dag_t* d, void* const* y, size_t* n_out);
 int    lrb200_dag_reset(lrb200_dag_t* d);
 const char* lrb200_dag_describe(const lrb200_dag_t* d);
 void   lrb200_dag_destroy(lrb200_dag_t* d);

@@ -131,6 +131,14 @@ return function (radio)
     end
     radio.IQFileSource.process = source_process(lib.lrb200_iqconv_create, "iqconv")
     radio.RealFileSource.process = source_process(lib.lrb200_realconv_create, "realconv")
+    -- a source read by a device DAG alone is absorbed into it: the converter is the DAG's first node (composite_patch.lua)
+    local function converter(self, create, what)
+        local h = create(self.format_name, b200.DEVICE)
+        if h == nil then b200.fail("Creating lrb200 " .. what .. " object") end
+        return h
+    end
+    function radio.IQFileSource:make_converter_handle() return converter(self, lib.lrb200_iqconv_create, "iqconv") end
+    function radio.RealFileSource:make_converter_handle() return converter(self, lib.lrb200_realconv_create, "realconv") end
     -- Sinks (radio/blocks/sinks/iqfile.lua:66-88, realfile.lua, wavfile.lua:170-194 for one channel): convert, then fwrite.
     local function sink_process(create, what)
         return function (self, x)

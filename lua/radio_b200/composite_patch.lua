@@ -5,7 +5,8 @@
 -- MAXIMAL LINEAR RUN of GPU blocks in the crawled connection graph is collapsed into ONE lrb200 flow graph:
 -- one process() call per source vector, device-resident intermediates, fused kernels, H2D/D2H only at the
 -- two ends of the run.  Before that, every connected NON-linear set of GPU blocks with a single outside feed (the WBFM
--- stereo demodulator: two-input blocks, the PLL's two outputs, fan-outs) becomes ONE device DAG (GPUDagBlock, lrb200_dag_*).
+-- stereo demodulator: two-input blocks, the PLL's two outputs, fan-outs) becomes ONE device DAG (GPUDagBlock, lrb200_dag_*),
+-- with the raw file source that feeds it alone absorbed as its first node.
 -- CPU blocks, and multi-input blocks or fan-out points outside such a set, stay ordinary blocks at the edges.
 --
 --   local top = radio.CompositeBlock(); top:connect(...); top:run()   -- unchanged user code
@@ -18,7 +19,7 @@
 --   _prepare_to_run (composite.lua:426-466)     hands the global evaluation order to the substitutes (EOF flush)
 --   start (composite.lua:534-545)               forces multiprocess = false
 -- Set LUARADIO_B200_SUPERCHUNK=<samples> to pack the per-vector calls into pinned super-chunks
--- (lrb200_graph_set_superchunk): throughput of the reference's 8192-sample vectors goes from launch-bound to
+-- (lrb200_graph_set_superchunk, lrb200_dag_set_superchunk): throughput of the reference's 8192-sample vectors goes from launch-bound to
 -- memcpy-bound; outputs then arrive in bursts, and the last partial super-chunk is only pushed out by cleanup().
 
 local ffi = require('ffi')
@@ -63,14 +64,16 @@ function GPUChainBlock:process(x)
     return out:resize(tonumber(n_out[0]))
 end
 
-function GPUChainBlock:cleanup()
-    -- super-chunk mode: hand the pending samples to the downstream pipes before they are closed
-    local lib = platform.libs.cuda
-    local out = self.out:resize(tonumber(lib.lrb200_graph_max_output(self.graph, 0)))
-    if lib.lrb200_graph_flush(self.graph, out.data, n_out) ~= 0 then b200.fail("graph_flush") end
-    out:resize(tonumber(n_out[0]))
-    if out.length > 0 then
-        for _, p in ipairs(self.outputs[1].pipes) do p:write(out) end
+--- Hand flushed super-chunk outputs (outs[k] for output port k) to the downstream pipes before they are closed.
+local function hand_on_flushed(self, outs)
+    local any = false
+    for k, out in ipairs(outs) do
+        if out.length > 0 then
+            any = true
+            for _, p in ipairs(self.outputs[k].pipes) do p:write(out) end
+        end
+    end
+    if any then
         -- The run loop has already ended (the source's EOF stops it at once, composite.lua:662-681) and cleanup() runs in
         -- evaluation order, so the blocks downstream are still alive: let each of them take one more turn on the flushed tail.
         local downstream, todo = {}, {self}
@@ -90,6 +93,14 @@ function GPUChainBlock:cleanup()
             if downstream[b] then b:run_once() end
         end
     end
+end
+
+function GPUChainBlock:cleanup()
+    -- super-chunk mode: hand the pending samples to the downstream pipes before they are closed
+    local lib = platform.libs.cuda
+    local out = self.out:resize(tonumber(lib.lrb200_graph_max_output(self.graph, 0)))
+    if lib.lrb200_graph_flush(self.graph, out.data, n_out) ~= 0 then b200.fail("graph_flush") end
+    hand_on_flushed(self, {out:resize(tonumber(n_out[0]))})
 end
 
 local M = {GPUChainBlock = GPUChainBlock}
@@ -159,14 +170,17 @@ end
 -- ONE outside output port, as one device DAG (lrb200_dag_*): every edge between the members is a device buffer, the only
 -- host traffic is the set's input and its outputs.  Linear runs inside the set become fused flow graphs
 -- (lrb200_dag_add_graph), everything else single nodes (lrb200_dag_add_block).  A node's output k is referenced as
--- node * 4 + k, the DAG's own input as -1 (include/lrb200.h).
+-- node * 4 + k, the DAG's own input as -1 (include/lrb200.h).  An absorbed raw file source (IQFileSource, RealFileSource
+-- read by the set alone) makes it a source block: it freads the file's bytes itself and the source's converter is the
+-- DAG's first node.  LUARADIO_B200_SUPERCHUNK switches on super-chunk mode (lrb200_dag_set_superchunk) as for the chains.
 local GPUDagBlock = block.factory("GPUDagBlock")
+GPUDagBlock.RAW_READ = 524288            -- samples per fread from an absorbed source (the reference's 8192 is launch-bound)
 
-function GPUDagBlock:instantiate(members, ext_in, ext_out, edges)
-    self.blocks, self.ext_in, self.ext_out, self.edges = members, ext_in, ext_out, edges
+function GPUDagBlock:instantiate(members, ext_in, ext_out, edges, raw_source)
+    self.blocks, self.ext_in, self.ext_out, self.edges, self.raw_source = members, ext_in, ext_out, edges, raw_source
     local outputs = {}
     for k, p in ipairs(ext_out) do outputs[k] = block.Output("out" .. k, p.data_type) end
-    self:add_type_signature({block.Input("in", ext_in.data_type)}, outputs)
+    self:add_type_signature(raw_source and {} or {block.Input("in", ext_in.data_type)}, outputs)
 end
 
 function GPUDagBlock:get_rate()
@@ -192,6 +206,16 @@ function GPUDagBlock:initialize()
     end
     local ref, done = {}, {}
     ref[self.ext_in] = -1
+    if self.raw_source then                               -- node 0: the file format converter, fed the raw bytes
+        local h = self.raw_source:make_converter_handle()
+        local ins = ffi.new("int[?]", 1)
+        ins[0] = -1
+        if lib.lrb200_dag_add_block(self.dag, h, ins, 1) < 0 then
+            lib.lrb200_block_destroy(h)
+            b200.fail("dag_add_block")
+        end
+        ref[self.ext_in] = 0
+    end
     for _, b in ipairs(self.blocks) do                    -- evaluation (topological) order
         if not done[b] then
             local run = {}
@@ -234,18 +258,48 @@ function GPUDagBlock:initialize()
     local outs = ffi.new("int[?]", #self.ext_out)
     for k, p in ipairs(self.ext_out) do outs[k - 1] = ref[p] end
     if lib.lrb200_dag_set_outputs(self.dag, outs, #self.ext_out) ~= 0 then b200.fail("dag_set_outputs") end
+    self.superchunk = tonumber(os.getenv('LUARADIO_B200_SUPERCHUNK') or 0)
+    if self.superchunk > 0 and lib.lrb200_dag_set_superchunk(self.dag, self.superchunk) ~= 0 then b200.fail("dag_set_superchunk") end
+    self.fed = false                                      -- samples went in since the last flush (super-chunk mode)
     self.outs, self.out_ptrs, self.n_outs = {}, ffi.new("void*[?]", #self.ext_out), ffi.new("size_t[?]", #self.ext_out)
     for k, p in ipairs(self.ext_out) do self.outs[k] = p.data_type.vector() end
+    -- the source was initialised with the original blocks (its file is open); read bigger chunks than its own
+    if self.raw_source then self.raw_source.raw_samples:resize(math.max(self.raw_source.chunk_size or 0, self.RAW_READ)) end
+end
+
+function GPUDagBlock:execute(data, n, flush)
+    local lib = platform.libs.cuda
+    for k, o in ipairs(self.outs) do
+        self.out_ptrs[k - 1] = o:resize(tonumber(lib.lrb200_dag_max_output(self.dag, k - 1, n))).data
+    end
+    if flush then
+        if lib.lrb200_dag_flush(self.dag, self.out_ptrs, self.n_outs) ~= 0 then b200.fail("dag_flush") end
+    elseif lib.lrb200_dag_execute(self.dag, data, n, self.out_ptrs, self.n_outs) ~= 0 then
+        b200.fail("dag_execute")
+    end
+    self.fed = self.superchunk > 0 and not flush
+    for k, o in ipairs(self.outs) do o:resize(tonumber(self.n_outs[k - 1])) end
+    return unpack(self.outs)
 end
 
 function GPUDagBlock:process(x)
-    local lib = platform.libs.cuda
-    for k, o in ipairs(self.outs) do
-        self.out_ptrs[k - 1] = o:resize(tonumber(lib.lrb200_dag_max_output(self.dag, k - 1, x.length))).data
+    if self.raw_source then
+        local src = self.raw_source
+        local n = tonumber(ffi.C.fread(src.raw_samples.data, ffi.sizeof(src.raw_samples.data_type), src.raw_samples.length, src.file))
+        if n == 0 then
+            if ffi.C.feof(src.file) ~= 0 and src.repeat_on_eof then ffi.C.rewind(src.file) else return nil end
+        end
+        return self:execute(src.raw_samples.data, n)
     end
-    if lib.lrb200_dag_execute(self.dag, x.data, x.length, self.out_ptrs, self.n_outs) ~= 0 then b200.fail("dag_execute") end
-    for k, o in ipairs(self.outs) do o:resize(tonumber(self.n_outs[k - 1])) end
-    return unpack(self.outs)
+    return self:execute(x.data, x.length)
+end
+
+function GPUDagBlock:cleanup()
+    -- super-chunk mode: hand the pending samples of every port to the downstream pipes before they are closed
+    if self.fed then
+        self:execute(nil, 0, true)
+        hand_on_flushed(self, self.outs)
+    end
 end
 
 M.GPUDagBlock = GPUDagBlock
@@ -341,6 +395,7 @@ function M.plan_gpu_dags(connections)
 end
 
 --- Substitute every planned set by one GPUDagBlock in the crawled connection map (before the linear runs are collapsed).
+-- A raw file source whose output only the set reads is absorbed (the rule CompositeBlock._collapse_gpu_runs applies).
 function M.collapse_gpu_dags(connections, substitutes)
     local plans = M.plan_gpu_dags(connections)
     for _, plan in ipairs(plans) do
@@ -349,8 +404,13 @@ function M.collapse_gpu_dags(connections, substitutes)
         for _, b in ipairs(plan.members) do
             for _, p in ipairs(b.inputs) do edges[p] = connections[p] end
         end
-        local dag = GPUDagBlock(plan.members, plan.ext_in, plan.ext_out, edges)
-        dag:differentiate({plan.ext_in.data_type})
+        local src = plan.ext_in.owner
+        if src.make_converter_handle == nil then src = nil end
+        for input, output in pairs(connections) do
+            if output == plan.ext_in and not member[input.owner] then src = nil end
+        end
+        local dag = GPUDagBlock(plan.members, plan.ext_in, plan.ext_out, edges, src)
+        dag:differentiate(src and {} or {plan.ext_in.data_type})
         if substitutes then substitutes[#substitutes + 1] = dag end
         -- outside readers of a member output now read the matching DAG output; the members' own edges disappear
         local rewire = {}
@@ -363,7 +423,7 @@ function M.collapse_gpu_dags(connections, substitutes)
         end
         for input, output in pairs(rewire) do connections[input] = output end
         for p, _ in pairs(edges) do connections[p] = nil end
-        connections[dag.inputs[1]] = plan.ext_in
+        if not src then connections[dag.inputs[1]] = plan.ext_in end
     end
     return connections
 end

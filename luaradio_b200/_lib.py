@@ -103,7 +103,10 @@ _PROTOS = {
     "lrb200_dag_add_graph": (c_int, [c_void_p, c_void_p, c_int]),
     "lrb200_dag_set_outputs": (c_int, [c_void_p, POINTER(c_int), c_uint]),
     "lrb200_dag_execute": (c_int, [c_void_p, c_void_p, c_size_t, POINTER(c_void_p), POINTER(c_size_t)]),
+    "lrb200_dag_execute_device": (c_int, [c_void_p, c_void_p, c_size_t, POINTER(c_void_p), POINTER(c_size_t)]),
     "lrb200_dag_max_output": (c_size_t, [c_void_p, c_uint, c_size_t]),
+    "lrb200_dag_set_superchunk": (c_int, [c_void_p, c_size_t]),
+    "lrb200_dag_flush": (c_int, [c_void_p, POINTER(c_void_p), POINTER(c_size_t)]),
     "lrb200_dag_reset": (c_int, [c_void_p]),
     "lrb200_dag_describe": (c_char_p, [c_void_p]),
     "lrb200_dag_destroy": (None, [c_void_p]),

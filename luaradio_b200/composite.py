@@ -577,8 +577,8 @@ class CompositeBlock(Block):
 
     def _collapse_gpu_runs(self, fuse, superchunk, device_dag=True):
         """Rewrite (self._all_connections, self._concrete_order): every planned device DAG becomes one GPUDagBlock, every
-        planned run one GPUChainBlock; a raw file source feeding only a run, and a raw file sink fed only by it, are absorbed
-        as its first / last stage."""
+        planned run one GPUChainBlock; a raw file source feeding only a run or a DAG, and a raw file sink fed only by a run,
+        are absorbed as its first / last stage."""
         orig = self._all_connections          # lookups use the untouched map; the rewrite goes into `conns`
         conns = dict(orig)
         consumers = {}
@@ -586,14 +586,18 @@ class CompositeBlock(Block):
             consumers.setdefault(outp, []).append(inp)
         chains, dag_members = [], set()
         for members, ext_in, ext_out in (self._plan_gpu_dags() if device_dag else []):
-            dag = GPUDagBlock(members, ext_in, ext_out, orig, fuse)
+            # a raw file source read by the DAG alone is absorbed: its converter becomes the DAG's first node
+            src = ext_in.owner if getattr(ext_in.owner, "raw_source", False) and \
+                all(cin.owner in members for cin in consumers.get(ext_in, [])) else None
+            dag = GPUDagBlock(members, ext_in, ext_out, orig, fuse, superchunk, src)
             chains.append(dag)
             dag_members.update(members)
             for m in members:
                 for p in m.inputs:
                     del conns[p]
-            conns[dag.inputs[0]] = ext_in
-            dag.inputs[0].pipe = next(p for m in members for p in m.inputs if orig[p] is ext_in).pipe
+            if src is None:
+                conns[dag.inputs[0]] = ext_in
+                dag.inputs[0].pipe = next(p for m in members for p in m.inputs if orig[p] is ext_in).pipe
             for k, port in enumerate(ext_out):
                 for cin in consumers.get(port, []):
                     if cin.owner not in dag_members:
@@ -629,8 +633,9 @@ class CompositeBlock(Block):
         return " ; ".join(c.desc for c in getattr(self, "_chains", []) if c.desc)
 
     def _schedule(self):
-        """One process, evaluation order, FIFOs per input port (composite.lua:647-707); at end of stream the chains are
-        flushed (super-chunk mode) and the graph drains."""
+        """One process, evaluation order, FIFOs per input port (composite.lua:647-707); at end of stream the chains and
+        DAGs are flushed (super-chunk mode) and the graph drains, again while a flush hands samples downstream (a device
+        sub-graph behind another one only sees the first one's tail after that drain)."""
         order, conns = self._run_order, self._run_connections
         fifo = {inp: [] for inp in conns}
         consumers = {}
@@ -645,7 +650,7 @@ class CompositeBlock(Block):
                 for cin in consumers.get(port, []):
                     fifo[cin].append(data)
 
-        exhausted, flushed = set(), False
+        exhausted, flushed, flush_moved = set(), False, False
         while not self._stop_requested:
             live = False
             for b in order:
@@ -672,15 +677,17 @@ class CompositeBlock(Block):
                 live = True
             if live:
                 continue
-            if flushed:
+            if flushed and not flush_moved:
                 break
             # every source is at EOF and nothing moved: push the pending super-chunks out and drain once more
-            flushed = True
+            flushed, flush_moved = True, False
             for b in order:
-                if isinstance(b, GPUChainBlock):
+                if isinstance(b, (GPUChainBlock, GPUDagBlock)):
                     r = b.flush()
                     if r is not None:
-                        push(b, (r,))
+                        outs = r if isinstance(r, tuple) else (r,)
+                        flush_moved = flush_moved or any(v is not None and v.length for v in outs)
+                        push(b, outs)
 
     def _run_body(self, fuse, superchunk, device_dag=True):
         try:
@@ -841,15 +848,20 @@ class GPUChainBlock(Block):
 class GPUDagBlock(Block):
     """A connected, non-linear set of GPU blocks as ONE device DAG (lrb200_dag_*): every edge between them is a device
     buffer; the only host traffic is the set's single input and its outputs.  Linear runs inside the set are added as fused
-    lrb200 flow graphs, the rest (two-input blocks, PLL, lone blocks) as single nodes."""
+    lrb200 flow graphs, the rest (two-input blocks, PLL, lone blocks) as single nodes.  An absorbed raw file source makes it
+    a source block: the file's own bytes cross PCIe and the source's converter is the DAG's first node.  With `superchunk`
+    the host vectors are packed into super-chunks (lrb200_dag_set_superchunk) and flush() drains them at end of stream."""
     name = "GPUDagBlock"
+    RAW_READ = GPUChainBlock.RAW_READ
 
-    def instantiate(self, members, ext_in, ext_out, connections, fuse=True):
+    def instantiate(self, members, ext_in, ext_out, connections, fuse=True, superchunk=0, raw_source=None):
         self.blocks, self.ext_in, self.ext_out, self.fuse = list(members), ext_in, list(ext_out), fuse
+        self.superchunk, self.raw_source = int(superchunk or 0), raw_source
         self._conn = connections
         self.dag, self.desc = None, ""
-        self.add_type_signature([Input("in", ext_in.data_type)], [Output("out%d" % (k + 1), p.data_type) for k, p in enumerate(ext_out)])
-        self.differentiate([ext_in.data_type])
+        ins = [] if raw_source is not None else [Input("in", ext_in.data_type)]
+        self.add_type_signature(ins, [Output("out%d" % (k + 1), p.data_type) for k, p in enumerate(ext_out)])
+        self.differentiate([d.data_type for d in ins])
 
     def get_rate(self):
         return self.ext_out[0].owner.get_rate()
@@ -862,6 +874,12 @@ class GPUDagBlock(Block):
         for inp, outp in conn.items():
             consumers.setdefault(outp, []).append(inp)
         ref = {self.ext_in: -1}                      # output port -> DAG reference
+        if self.raw_source is not None:              # node 0: the file format converter, fed the raw bytes
+            h = self.raw_source.make_device_handle()
+            if lib.lrb200_dag_add_block(d, h, (ctypes.c_int * 1)(-1), 1) < 0:
+                lib.lrb200_block_destroy(h)
+                raise _lib.LibraryError("dag_add_block(file source): " + _lib.last_error())
+            ref[self.ext_in] = 0
 
         def simple(b):
             return len(b.inputs) == 1 and len(b.outputs) == 1
@@ -902,21 +920,39 @@ class GPUDagBlock(Block):
             done.add(b)
         outs = (ctypes.c_int * len(self.ext_out))(*[ref[p] for p in self.ext_out])
         _lib.check(lib.lrb200_dag_set_outputs(d, outs, len(self.ext_out)), "dag_set_outputs")
+        if self.superchunk:
+            _lib.check(lib.lrb200_dag_set_superchunk(d, self.superchunk), "dag_set_superchunk")
         self.desc = "dag{" + lib.lrb200_dag_describe(d).decode() + "}"
         self.outs = [p.data_type.vector() for p in self.ext_out]
         self._n_out = (ctypes.c_size_t * len(self.ext_out))()
+        self._fed = False                            # samples went in since the last flush (super-chunk mode)
 
-    def process(self, x):
+    def _execute(self, in_ptr, n_in, flush=False):
         lib, d = self._lib, self.dag
         for k, o in enumerate(self.outs):
-            o.resize(lib.lrb200_dag_max_output(d, k, x.length))
+            o.resize(lib.lrb200_dag_max_output(d, k, n_in))
         ptrs = (ctypes.c_void_p * len(self.outs))(*[o.ctypes_ptr() for o in self.outs])
-        _lib.check(lib.lrb200_dag_execute(d, x.ctypes_ptr(), x.length, ptrs, self._n_out), "dag_execute")
+        if flush:
+            _lib.check(lib.lrb200_dag_flush(d, ptrs, self._n_out), "dag_flush")
+        else:
+            _lib.check(lib.lrb200_dag_execute(d, in_ptr, n_in, ptrs, self._n_out), "dag_execute")
+        self._fed = bool(self.superchunk) and not flush
         res = tuple(o.resize(self._n_out[k]) for k, o in enumerate(self.outs))
         return res[0] if len(res) == 1 else res
 
+    def process(self, x=None):
+        if self.raw_source is not None:
+            raw = self.raw_source.read_raw(max(self.raw_source.chunk_size, self.RAW_READ))
+            if raw is None:
+                return None                                   # EOF (block.lua:588)
+            return self._execute(raw.ctypes.data, len(raw) // self.raw_source.sample_bytes)
+        return self._execute(x.ctypes_ptr(), x.length)
+
     def flush(self):
-        return None
+        """The pending super-chunks' outputs, one vector per port (a vector when there is one port), or None."""
+        if not self.dag or not self._fed:
+            return None
+        return self._execute(None, 0, flush=True)
 
     def cleanup(self):
         if self.dag:

@@ -12,6 +12,7 @@
 #include <cmath>
 #include <cstdlib>
 #include <cstring>
+#include <functional>
 #include <memory>
 #include <new>
 #include <string>
@@ -166,6 +167,130 @@ static int fuse_iir_decimator(const Blocks& blocks, size_t i, Rewrite* out) {
 static const Rule FUSION_RULES[] = {fuse_tuner, fuse_rotator_overlap_save, fuse_interpolator, fuse_noble_identity,
                                    fuse_fir_decimator, fuse_iir_decimator};
 
+// Super-chunk mode (SURVEY.md 8e "streaming mode") of a linear graph or a DAG: small host vectors are packed into pinned
+// slots of `samples` input samples; a full slot is processed asynchronously while the next one fills, and its outputs (one
+// stream per output port) are handed back when that next slot is submitted (or at flush) -- the per-vector cost is one
+// host memcpy instead of copies + launches + a sync.  Every port's outputs come from the same slots.
+struct SuperChunk {
+    // device in / outs of one slot, asynchronous on s: dy[k] receives n_out[k] samples of port k
+    using Run = std::function<int(const void* dx, size_t n, void* const* dy, size_t* n_out, cudaStream_t s)>;
+    struct HostFree { void operator()(char* p) const { cudaFreeHost(p); } };
+    using PinnedSlot = std::unique_ptr<char, HostFree>;
+    size_t samples = 0;                     // input samples per slot; 0 = off
+    size_t in_size = 0;
+    std::vector<size_t> out_size, outcap;   // per port: bytes per sample, samples a slot can produce
+    PinnedSlot hin[2];
+    std::vector<PinnedSlot> hout[2];
+    DeviceBuffer din[2];
+    std::vector<DeviceBuffer> dout[2];
+    cudaEvent_t done[2] = {nullptr, nullptr};
+    bool pending[2] = {false, false};
+    std::vector<size_t> nout[2];
+    size_t fill = 0;
+    int cur = 0;
+
+    ~SuperChunk() { release(); }
+    bool busy() const { return pending[0] || pending[1] || fill; }
+    size_t ports() const { return out_size.size(); }
+
+    void release() {
+        for (int i = 0; i < 2; ++i) {
+            hin[i].reset(); hout[i].clear();
+            din[i] = DeviceBuffer(); dout[i].clear();
+            if (done[i]) cudaEventDestroy(done[i]);
+            done[i] = nullptr;
+            pending[i] = false; nout[i].clear();
+        }
+        samples = 0; fill = 0; cur = 0;
+    }
+    // `cap[k]`: samples port k can produce from one slot of `samples` inputs
+    int configure(size_t n, size_t isz, const std::vector<size_t>& osz, const std::vector<size_t>& cap) {
+        release();
+        if (n == 0) return 0;
+        in_size = isz; out_size = osz; outcap = cap;
+        for (int i = 0; i < 2; ++i) {
+            char* p = nullptr;
+            LRB_CHECK(cudaHostAlloc((void**)&p, n * isz, cudaHostAllocDefault));
+            hin[i].reset(p);
+            if (din[i].reserve(n * isz) != 0) return -1;
+            hout[i].resize(ports());
+            dout[i].resize(ports());
+            nout[i].assign(ports(), 0);
+            for (size_t k = 0; k < ports(); ++k) {
+                LRB_CHECK(cudaHostAlloc((void**)&p, cap[k] * osz[k], cudaHostAllocDefault));
+                hout[i][k].reset(p);
+                if (dout[i][k].reserve(cap[k] * osz[k]) != 0) return -1;
+            }
+            LRB_CHECK(cudaEventCreateWithFlags(&done[i], cudaEventDisableTiming));
+        }
+        samples = n;
+        return 0;
+    }
+    // wait for the slots in flight and forget them and the partial slot
+    int drop() {
+        for (int i = 0; i < 2; ++i) {
+            if (pending[i] && !cuda_ok(cudaEventSynchronize(done[i]), "cudaEventSynchronize")) return -1;
+            pending[i] = false;
+        }
+        fill = 0; cur = 0;
+        return 0;
+    }
+    // append a finished slot's outputs to y[k] + produced[k]
+    int collect(int slot, char* const* y, size_t* produced) {
+        if (!pending[slot]) return 0;
+        if (!cuda_ok(cudaEventSynchronize(done[slot]), "cudaEventSynchronize")) return -1;
+        for (size_t k = 0; k < ports(); ++k) {
+            if (nout[slot][k]) memcpy(y[k] + produced[k] * out_size[k], hout[slot][k].get(), nout[slot][k] * out_size[k]);
+            produced[k] += nout[slot][k];
+        }
+        pending[slot] = false;
+        return 0;
+    }
+    int submit(int slot, size_t count, const Run& run) {
+        cudaStream_t s = ctx().stream;
+        std::vector<void*> dy(ports());
+        for (size_t k = 0; k < ports(); ++k) dy[k] = dout[slot][k].get();
+        LRB_CHECK(cudaMemcpyAsync(din[slot].get(), hin[slot].get(), count * in_size, cudaMemcpyHostToDevice, s));
+        if (run(din[slot].get(), count, dy.data(), nout[slot].data(), s) != 0) return -1;
+        for (size_t k = 0; k < ports(); ++k)
+            if (nout[slot][k])
+                LRB_CHECK(cudaMemcpyAsync(hout[slot][k].get(), dy[k], nout[slot][k] * out_size[k], cudaMemcpyDeviceToHost, s));
+        LRB_CHECK(cudaEventRecord(done[slot], s));
+        pending[slot] = true;
+        return 0;
+    }
+    int accumulate(const void* x, size_t n, char* const* y, size_t* n_out, const Run& run) {
+        const char* xp = (const char*)x;
+        for (size_t k = 0; k < ports(); ++k) n_out[k] = 0;
+        while (n > 0) {
+            const size_t take = n < samples - fill ? n : samples - fill;
+            memcpy(hin[cur].get() + fill * in_size, xp, take * in_size);
+            fill += take; xp += take * in_size; n -= take;
+            if (fill == samples) {
+                // the other slot was submitted one super-chunk ago: its results are (long) ready
+                if (collect(cur ^ 1, y, n_out) != 0) return -1;
+                if (submit(cur, samples, run) != 0) return -1;
+                cur ^= 1;
+                fill = 0;
+            }
+        }
+        return 0;
+    }
+    int flush(char* const* y, size_t* n_out, const Run& run) {
+        for (size_t k = 0; k < ports(); ++k) n_out[k] = 0;
+        if (!samples) return 0;
+        if (collect(cur ^ 1, y, n_out) != 0) return -1;
+        if (fill) {
+            if (submit(cur, fill, run) != 0) return -1;
+            if (collect(cur, y, n_out) != 0) return -1;
+            fill = 0;
+        }
+        return 0;
+    }
+    // room one call appending n samples may need in port k
+    size_t max_output(size_t k, size_t n) const { return (n / samples + 2) * outcap[k]; }
+};
+
 // A committed linear run of blocks, itself a one-port Block (a node of a Dag).  Its name is the description.
 struct Graph : Block {
     Blocks blocks;                   // as appended
@@ -178,19 +303,7 @@ struct Graph : Block {
     cudaStream_t s_h2d = nullptr, s_d2h = nullptr;
     cudaEvent_t ev_h2d[2] = {nullptr, nullptr}, ev_comp[2] = {nullptr, nullptr}, ev_d2h[2] = {nullptr, nullptr};
     size_t host_chunk = (size_t)1 << 23;   // input samples per pipelined chunk
-    // super-chunk mode (SURVEY.md 8e "streaming mode"): small host vectors are packed into pinned slots of `sc` samples;
-    // a full slot is processed asynchronously while the next one fills, and its outputs are handed back when that next
-    // slot is submitted (or at flush) -- the per-vector cost is one host memcpy instead of copies + launches + a sync
-    struct HostFree { void operator()(char* p) const { cudaFreeHost(p); } };
-    using PinnedSlot = std::unique_ptr<char, HostFree>;
-    size_t sc = 0;
-    PinnedSlot sc_hin[2], sc_hout[2];
-    DeviceBuffer sc_din[2], sc_dout[2];
-    cudaEvent_t sc_done[2] = {nullptr, nullptr};
-    bool sc_pending[2] = {false, false};
-    size_t sc_nout[2] = {0, 0};
-    size_t sc_fill = 0, sc_outcap = 0;
-    int sc_cur = 0;
+    SuperChunk sc;                   // super-chunk mode (lrb200_graph_set_superchunk)
     // time-chunk sharding (run_shard): scratch for the outputs that belong to the halo
     DeviceBuffer head_out;
     // optional per-stage timing
@@ -226,18 +339,6 @@ struct Graph : Block {
         }
         if (s_h2d) cudaStreamDestroy(s_h2d);
         if (s_d2h) cudaStreamDestroy(s_d2h);
-        free_superchunk();
-    }
-
-    void free_superchunk() {
-        for (int i = 0; i < 2; ++i) {
-            sc_hin[i].reset(); sc_hout[i].reset();
-            sc_din[i] = DeviceBuffer(); sc_dout[i] = DeviceBuffer();
-            if (sc_done[i]) cudaEventDestroy(sc_done[i]);
-            sc_done[i] = nullptr;
-            sc_pending[i] = false; sc_nout[i] = 0;
-        }
-        sc = 0; sc_fill = 0; sc_cur = 0;
     }
 
     size_t max_output(size_t n) const override {
@@ -343,7 +444,7 @@ struct Graph : Block {
         if (stages.empty()) { set_error("graph: no blocks"); return -1; }
         cudaStream_t s = ctx().stream;
         const size_t isz = in_size, osz = out_size;
-        if (sc) return run_accumulate(x, n, y, n_out);
+        if (sc.samples) return sc.accumulate(x, n, (char* const*)&y, n_out, sc_run());
         if (n <= host_chunk) {
             // one chunk (every call of the reference's per-vector regime, pipe.lua:73): copy, kernels and copy back in
             // order on ONE stream with ONE synchronize -- no cross-stream events, nothing to overlap anyway
@@ -394,87 +495,16 @@ struct Graph : Block {
     }
 
     // ---- super-chunk mode -------------------------------------------------------------------------------------
+    SuperChunk::Run sc_run() {
+        return [this](const void* dx, size_t n, void* const* dy, size_t* n_out, cudaStream_t s) { return run(dx, n, dy[0], n_out, s); };
+    }
     int set_superchunk(size_t samples) {
         if (ensure_committed() != 0) return -1;
         if (stages.empty()) { set_error("graph: no blocks"); return -1; }
-        if (sc_pending[0] || sc_pending[1] || sc_fill) { set_error("graph: flush before changing the super-chunk size"); return -1; }
-        free_superchunk();
-        if (samples == 0) return 0;
-        const size_t isz = in_size, osz = out_size;
-        sc_outcap = max_output(samples) + 1;
-        for (int i = 0; i < 2; ++i) {
-            char* p = nullptr;
-            LRB_CHECK(cudaHostAlloc((void**)&p, samples * isz, cudaHostAllocDefault));
-            sc_hin[i].reset(p);
-            LRB_CHECK(cudaHostAlloc((void**)&p, sc_outcap * osz, cudaHostAllocDefault));
-            sc_hout[i].reset(p);
-            if (sc_din[i].reserve(samples * isz) != 0 || sc_dout[i].reserve(sc_outcap * osz) != 0) return -1;
-            LRB_CHECK(cudaEventCreateWithFlags(&sc_done[i], cudaEventDisableTiming));
-        }
-        sc = samples;
-        return 0;
+        if (sc.busy()) { set_error("graph: flush before changing the super-chunk size"); return -1; }
+        return sc.configure(samples, in_size, {out_size}, {max_output(samples) + 1});
     }
-    size_t sc_collect(int slot, char* y) {
-        if (!sc_pending[slot]) return 0;
-        if (!cuda_ok(cudaEventSynchronize(sc_done[slot]), "cudaEventSynchronize")) return (size_t)-1;
-        const size_t osz = out_size;
-        if (sc_nout[slot]) memcpy(y, sc_hout[slot].get(), sc_nout[slot] * osz);
-        sc_pending[slot] = false;
-        return sc_nout[slot];
-    }
-    int sc_submit(int slot, size_t count) {
-        cudaStream_t s = ctx().stream;
-        const size_t isz = in_size, osz = out_size;
-        size_t no = 0;
-        LRB_CHECK(cudaMemcpyAsync(sc_din[slot].get(), sc_hin[slot].get(), count * isz, cudaMemcpyHostToDevice, s));
-        if (run(sc_din[slot].get(), count, sc_dout[slot].get(), &no, s) != 0) return -1;
-        if (no) LRB_CHECK(cudaMemcpyAsync(sc_hout[slot].get(), sc_dout[slot].get(), no * osz, cudaMemcpyDeviceToHost, s));
-        LRB_CHECK(cudaEventRecord(sc_done[slot], s));
-        sc_nout[slot] = no;
-        sc_pending[slot] = true;
-        return 0;
-    }
-    int run_accumulate(const void* x, size_t n, void* y, size_t* n_out) {
-        const size_t isz = in_size, osz = out_size;
-        const char* xp = (const char*)x;
-        char* yp = (char*)y;
-        size_t produced = 0;
-        while (n > 0) {
-            const size_t take = n < sc - sc_fill ? n : sc - sc_fill;
-            memcpy(sc_hin[sc_cur].get() + sc_fill * isz, xp, take * isz);
-            sc_fill += take; xp += take * isz; n -= take;
-            if (sc_fill == sc) {
-                // the other slot was submitted one super-chunk ago: its results are (long) ready
-                const size_t got = sc_collect(sc_cur ^ 1, yp + produced * osz);
-                if (got == (size_t)-1) return -1;
-                produced += got;
-                if (sc_submit(sc_cur, sc) != 0) return -1;
-                sc_cur ^= 1;
-                sc_fill = 0;
-            }
-        }
-        *n_out = produced;
-        return 0;
-    }
-    int flush(void* y, size_t* n_out) {
-        *n_out = 0;
-        if (!sc) return 0;
-        const size_t osz = out_size;
-        char* yp = (char*)y;
-        size_t produced = 0;
-        size_t got = sc_collect(sc_cur ^ 1, yp);
-        if (got == (size_t)-1) return -1;
-        produced += got;
-        if (sc_fill) {
-            if (sc_submit(sc_cur, sc_fill) != 0) return -1;
-            got = sc_collect(sc_cur, yp + produced * osz);
-            if (got == (size_t)-1) return -1;
-            produced += got;
-            sc_fill = 0;
-        }
-        *n_out = produced;
-        return 0;
-    }
+    int flush(void* y, size_t* n_out) { return sc.flush((char* const*)&y, n_out, sc_run()); }
 
     // Block::reset for every block, with ONE launch zeroing the carried state of them all
     int reset(cudaStream_t s) {
@@ -621,7 +651,8 @@ struct Graph : Block {
 // DAG's own input.  Every edge is a grow-only device buffer; all inputs of a node must deliver the same number of samples
 // per call (true whenever the converging paths have the same rate changes -- every block here is zero-latency; the
 // reference's PipeMux would buffer a surplus instead, radio/core/pipe.lua:495-615).  Host in, host out(s): one upload,
-// the node launches in order on the library stream, one download per output, one synchronize.
+// the node launches in order on the library stream, one download per output, one synchronize; or the same launches on
+// device-resident input and outputs with no synchronize; or host vectors packed into super-chunks (SuperChunk above).
 // This is what composites/wbfmstereodemodulator.lua:22-64 and amsynchronousdemodulator.lua:25-45 need on the device.
 // ---------------------------------------------------------------------------------------------------------------------
 struct DagNode {
@@ -629,6 +660,7 @@ struct DagNode {
     std::vector<int> in_refs;      // producer node * 4 + port, or -1 for the DAG input
     std::vector<DeviceBuffer> out_buf;
     std::vector<size_t> out_cnt;
+    std::vector<void*> out_ptr;    // where each port's samples of the current call are (out_buf, or a caller's dy)
 };
 
 struct Dag {
@@ -637,6 +669,8 @@ struct Dag {
     DeviceBuffer d_in;
     size_t in_size = 0;
     std::string desc;
+    SuperChunk sc;                 // super-chunk mode (lrb200_dag_set_superchunk)
+    bool sc_fed = false;           // an execute since super-chunk mode was set, or since the last flush / reset
 
     // on success the DAG owns blk; on failure the caller keeps it
     int add(Block* blk, const int* refs, unsigned nin) {
@@ -645,6 +679,7 @@ struct Dag {
         if (wire(nd, refs, nin) != 0) { nd.blk.release(); return -1; }
         nd.out_buf.resize((size_t)blk->num_outputs);
         nd.out_cnt.assign((size_t)blk->num_outputs, 0);
+        nd.out_ptr.assign((size_t)blk->num_outputs, nullptr);
         if (!desc.empty()) desc += " ; ";
         desc += blk->name;
         nodes.push_back(std::move(nd));
@@ -672,28 +707,39 @@ struct Dag {
         return 0;
     }
 
+    size_t out_size(size_t k) const { return nodes[(size_t)(outputs[k] >> 2)].blk->out_size_of(outputs[k] & 3); }
+    // conservative: no node here produces more samples than its input times the interpolation factors on the way
+    size_t max_output(size_t n) const {
+        size_t m = n;
+        for (const DagNode& nd : nodes) { const size_t c = nd.blk->max_output(n); if (c > m) m = c; }
+        return m;
+    }
+
+    // back to the state after creation: the slots in flight are waited for and dropped with the partial slot (the
+    // super-chunk size stays), then every node's carried state is zeroed
     int reset() {
+        if (sc.drop() != 0) return -1;
+        sc_fed = false;
         for (DagNode& nd : nodes)
             if (nd.blk->reset() != 0) return -1;
         return 0;
     }
 
-    int run_host(const void* x, size_t n, void* const* y, size_t* n_out) {
+    // The node launches of one call, asynchronous on s: the DAG input is dx (n samples, device).  With dy, output k's
+    // n_out[k] samples go to dy[k] (the producing node writes there, and its consumers read them there); without, they
+    // stay in the producer's edge buffer.  Every count is host arithmetic, so nothing here synchronizes except growing
+    // an edge buffer.
+    int run_nodes(const void* dx, size_t n, void* const* dy, size_t* n_out, cudaStream_t s) {
         if (nodes.empty() || outputs.empty()) { set_error("dag: no nodes / no outputs"); return -1; }
-        cudaStream_t s = ctx().stream;
-        if (n * in_size > d_in.capacity()) {
-            LRB_CHECK(cudaStreamSynchronize(s));
-            if (d_in.reserve(n * in_size) != 0) return -1;
-        }
-        if (n) LRB_CHECK(cudaMemcpyAsync(d_in.get(), x, n * in_size, cudaMemcpyHostToDevice, s));
-        for (DagNode& nd : nodes) {
+        for (size_t i = 0; i < nodes.size(); ++i) {
+            DagNode& nd = nodes[i];
             std::vector<const void*> ins;
             size_t cnt = 0;
-            for (size_t i = 0; i < nd.in_refs.size(); ++i) {
-                const int r = nd.in_refs[i];
-                const void* p = r == -1 ? d_in.get() : nodes[(size_t)(r >> 2)].out_buf[(size_t)(r & 3)].get();
+            for (size_t j = 0; j < nd.in_refs.size(); ++j) {
+                const int r = nd.in_refs[j];
+                const void* p = r == -1 ? dx : nodes[(size_t)(r >> 2)].out_ptr[(size_t)(r & 3)];
                 const size_t c = r == -1 ? n : nodes[(size_t)(r >> 2)].out_cnt[(size_t)(r & 3)];
-                if (i && c != cnt) { set_error("dag: %s received inputs of different lengths (%zu, %zu)", nd.blk->name.c_str(), cnt, c); return -1; }
+                if (j && c != cnt) { set_error("dag: %s received inputs of different lengths (%zu, %zu)", nd.blk->name.c_str(), cnt, c); return -1; }
                 cnt = c;
                 ins.push_back(p);
             }
@@ -701,13 +747,20 @@ struct Dag {
             const size_t mo = nd.blk->max_output(cnt);
             void* outs[4];                 // a port is two bits of a reference
             for (int o = 0; o < nout; ++o) {
-                DeviceBuffer& buf = nd.out_buf[(size_t)o];
-                const size_t bytes = (mo ? mo : 1) * nd.blk->out_size_of(o);
-                if (bytes > buf.capacity()) {
-                    LRB_CHECK(cudaStreamSynchronize(s));
-                    if (buf.reserve(bytes) != 0) return -1;
+                const int ref = (int)i * 4 + o;
+                void* ext = nullptr;
+                for (size_t k = 0; dy && k < outputs.size() && !ext; ++k)
+                    if (outputs[k] == ref) ext = dy[k];
+                if (!ext) {
+                    DeviceBuffer& buf = nd.out_buf[(size_t)o];
+                    const size_t bytes = (mo ? mo : 1) * nd.blk->out_size_of(o);
+                    if (bytes > buf.capacity()) {
+                        LRB_CHECK(cudaStreamSynchronize(s));
+                        if (buf.reserve(bytes) != 0) return -1;
+                    }
+                    ext = buf.get();
                 }
-                outs[o] = buf.get();
+                outs[o] = nd.out_ptr[(size_t)o] = ext;
             }
             size_t no = 0;
             if (nd.blk->run_multi(ins.data(), (int)ins.size(), cnt, outs, nout, &no, s) != 0) return -1;
@@ -715,13 +768,62 @@ struct Dag {
         }
         for (size_t k = 0; k < outputs.size(); ++k) {
             const DagNode& nd = nodes[(size_t)(outputs[k] >> 2)];
-            const int port = outputs[k] & 3;
-            const size_t c = nd.out_cnt[(size_t)port];
-            if (c) LRB_CHECK(cudaMemcpyAsync(y[k], nd.out_buf[(size_t)port].get(), c * nd.blk->out_size_of(port), cudaMemcpyDeviceToHost, s));
+            const size_t port = (size_t)(outputs[k] & 3), c = nd.out_cnt[port];
+            // an output listed twice: the producer wrote the first dy only
+            if (dy && c && nd.out_ptr[port] != dy[k])
+                LRB_CHECK(cudaMemcpyAsync(dy[k], nd.out_ptr[port], c * out_size(k), cudaMemcpyDeviceToDevice, s));
             n_out[k] = c;
+        }
+        return 0;
+    }
+
+    SuperChunk::Run sc_run() {
+        return [this](const void* dx, size_t n, void* const* dy, size_t* n_out, cudaStream_t s) { return run_nodes(dx, n, dy, n_out, s); };
+    }
+
+    // host in, host outs: one upload, the node launches, one download per output, one synchronize -- or, in super-chunk
+    // mode, the vector appended to the current slot
+    int run_host(const void* x, size_t n, void* const* y, size_t* n_out) {
+        if (nodes.empty() || outputs.empty()) { set_error("dag: no nodes / no outputs"); return -1; }
+        if (sc.samples) {
+            sc_fed = true;
+            return sc.accumulate(x, n, (char* const*)y, n_out, sc_run());
+        }
+        cudaStream_t s = ctx().stream;
+        if (n * in_size > d_in.capacity()) {
+            LRB_CHECK(cudaStreamSynchronize(s));
+            if (d_in.reserve(n * in_size) != 0) return -1;
+        }
+        if (n) LRB_CHECK(cudaMemcpyAsync(d_in.get(), x, n * in_size, cudaMemcpyHostToDevice, s));
+        if (run_nodes(d_in.get(), n, nullptr, n_out, s) != 0) return -1;
+        for (size_t k = 0; k < outputs.size(); ++k) {
+            const DagNode& nd = nodes[(size_t)(outputs[k] >> 2)];
+            if (n_out[k]) LRB_CHECK(cudaMemcpyAsync(y[k], nd.out_ptr[(size_t)(outputs[k] & 3)], n_out[k] * out_size(k), cudaMemcpyDeviceToHost, s));
         }
         LRB_CHECK(cudaStreamSynchronize(s));
         return 0;
+    }
+
+    int run_device(const void* dx, size_t n, void* const* dy, size_t* n_out) {
+        if (sc.samples) { set_error("dag: execute_device runs the stream directly; switch super-chunk mode off first (set_superchunk 0)"); return -1; }
+        return run_nodes(dx, n, dy, n_out, ctx().stream);
+    }
+
+    int set_superchunk(size_t samples) {
+        if (nodes.empty() || outputs.empty()) { set_error("dag: no nodes / no outputs"); return -1; }
+        if (sc.busy()) { set_error("dag: flush before changing the super-chunk size"); return -1; }
+        std::vector<size_t> osz, cap;
+        for (size_t k = 0; k < outputs.size(); ++k) { osz.push_back(out_size(k)); cap.push_back(max_output(samples) + 1); }
+        sc_fed = false;
+        return sc.configure(samples, in_size, osz, cap);
+    }
+
+    int flush(void* const* y, size_t* n_out) {
+        for (size_t k = 0; k < outputs.size(); ++k) n_out[k] = 0;
+        if (!sc.samples) { set_error("dag: flush needs super-chunk mode (set_superchunk)"); return -1; }
+        if (!sc_fed) { set_error("dag: nothing to flush: no execute since super-chunk mode was set, the last flush or reset"); return -1; }
+        sc_fed = false;
+        return sc.flush((char* const*)y, n_out, sc_run());
     }
 };
 
@@ -785,7 +887,7 @@ size_t lrb200_graph_max_output(const lrb200_graph_t* g, size_t n) {
     Graph& gr = *g->g;
     if (gr.ensure_committed() != 0) return 0;
     // super-chunk mode: one call may hand back the results of the slots completed while n samples were appended
-    if (gr.sc) return (n / gr.sc + 2) * gr.sc_outcap;
+    if (gr.sc.samples) return gr.sc.max_output(0, n);
     return gr.max_output(n);
 }
 
@@ -902,6 +1004,7 @@ int lrb200_dag_add_graph(lrb200_dag_t* d, lrb200_graph_t* g, int input) {
 
 int lrb200_dag_set_outputs(lrb200_dag_t* d, const int* outputs, unsigned num_outputs) {
     if (!d || !outputs || !num_outputs) { set_error("dag_set_outputs: null argument"); return -1; }
+    if (d->d.sc.samples) { set_error("dag_set_outputs: the super-chunk slots are sized for the outputs; set them first"); return -1; }
     for (unsigned k = 0; k < num_outputs; ++k) {
         const int r = outputs[k];
         if (r < 0 || (r >> 2) >= (int)d->d.nodes.size() || (r & 3) >= d->d.nodes[(size_t)(r >> 2)].blk->num_outputs) { set_error("dag_set_outputs: bad reference %d", r); return -1; }
@@ -915,12 +1018,26 @@ int lrb200_dag_execute(lrb200_dag_t* d, const void* x, size_t n, void* const* y,
     return d->d.run_host(x, n, y, n_out);
 }
 
+int lrb200_dag_execute_device(lrb200_dag_t* d, const void* dx, size_t n, void* const* dy, size_t* n_out) {
+    if (!d || !dy || !n_out || (n && !dx)) { set_error("dag_execute_device: null argument"); return -1; }
+    return d->d.run_device(dx, n, dy, n_out);
+}
+
 size_t lrb200_dag_max_output(const lrb200_dag_t* d, unsigned output, size_t n) {
     if (!d || output >= d->d.outputs.size()) return 0;
-    // conservative: no node here produces more samples than its input times the interpolation factors on the way
-    size_t m = n;
-    for (const DagNode& nd : d->d.nodes) { const size_t c = nd.blk->max_output(n); if (c > m) m = c; }
-    return m;
+    // super-chunk mode: one call may hand back the results of the slots completed while n samples were appended
+    if (d->d.sc.samples) return d->d.sc.max_output(output, n);
+    return d->d.max_output(n);
+}
+
+int lrb200_dag_set_superchunk(lrb200_dag_t* d, size_t samples) {
+    if (!d) { set_error("null dag"); return -1; }
+    return d->d.set_superchunk(samples);
+}
+
+int lrb200_dag_flush(lrb200_dag_t* d, void* const* y, size_t* n_out) {
+    if (!d || !y || !n_out) { set_error("dag_flush: null argument"); return -1; }
+    return d->d.flush(y, n_out);
 }
 
 int lrb200_dag_reset(lrb200_dag_t* d) {
