@@ -205,9 +205,10 @@ lrb200_block_t* lrb200_upsample_create(unsigned factor, unsigned elem_size, unsi
  * output 1 = phase error (Float32); execute through lrb200_block_execute_multi with one input and two outputs.  The
  * recurrence is nonlinear and is run in stream order by one thread (exact, a few MS/s).  lrb200_pll_set_mode(q, 1) opts
  * into the chunk-parallel form for long calls: each chunk is simulated by its own thread after a lead-in of
- * 24 / (zeta * loop bandwidth) samples from the phase of the input and the centre frequency, and the multiplied phase is
- * rebuilt exactly from prefix sums of the per-chunk phase increments and errors -- equal to the sequential recurrence (to
- * float32 resolution) WHILE THE LOOP IS LOCKED, not while it acquires or free-runs on noise. */
+ * 24 / (zeta * loop bandwidth) samples from the phase of the input and the centre frequency; the multiplied phase is
+ * carried across the chunks as per-chunk advances wrapped to +-2 pi at every step, as the sequential form wraps it, so
+ * its rounding does not grow with the call.  It equals the sequential recurrence to the resolution of the float32 phase
+ * detector WHILE THE LOOP IS LOCKED, not while it acquires or free-runs on noise. */
 lrb200_block_t* lrb200_binary_create(const char* op, unsigned complex_data, unsigned flags);
 lrb200_block_t* lrb200_pll_create(double loop_bandwidth, double frequency_min, double frequency_max, double multiplier,
                                   double rate, unsigned flags);

@@ -242,12 +242,14 @@ __global__ void pll_kernel(const float2* __restrict__ x, long long n, float2* __
 // arg(x) and the centre frequency the second-order loop converges to the stream's own (phi_locked, freq_locked)
 // trajectory within W = 24 / (zeta * loop bandwidth) samples, so every chunk can be simulated by its own thread after a
 // W-sample lead-in (chunk 0 starts from the carried state and is exact).  phi_multiplied is NOT a function of the locked
-// state (it integrates multiplier * freq + alpha * error over the whole past), so it is rebuilt exactly from prefix sums
-// over the chunks: with A[i] = sum_{k<i} (freq'_k + alpha e_k) and E[i] = sum_{k<i} e_k,
-//     phi_multiplied[i] = phi_multiplied[0] + m A[i] + (1 - m) alpha E[i]     (mod 2 pi).
-struct PllChunk { double freq0, dA, dE, phi_end, freq_end, A0, E0; };
+// state (it integrates multiplier * freq' + alpha * error over the whole past, freq' the frequency before the clamp), so
+// it is carried across the chunks instead: each chunk's advance dP is summed in the sequential kernel's own expression
+// and wrapped to +-2 pi at every step, the bases are summed and wrapped once per chunk, and the output pass advances
+// phi_multiplied from its chunk's base exactly as pll_kernel does.  Every partial sum stays below 4 pi, so the rounding
+// per sample is that of the sequential kernel: no sum grows with the call.
+struct PllChunk { double freq0, dP, phi_end, freq_end, base; };
 
-__device__ __forceinline__ float pll_step(float2 xv, double& phi, double& freq, const PllParams& P, double& inc) {
+__device__ __forceinline__ float pll_step(float2 xv, double& phi, double& freq, const PllParams& P) {
     const double two_pi = 6.283185307179586476925286766559;
     double s, c;
     sincos(phi, &s, &c);
@@ -255,14 +257,24 @@ __device__ __forceinline__ float pll_step(float2 xv, double& phi, double& freq, 
     const float pr = (float)((double)xv.x * (double)vr - (double)xv.y * (double)(-vi));
     const float pi = (float)((double)xv.x * (double)(-vi) + (double)xv.y * (double)vr);
     const float e = atan2f(pi, pr);
-    freq = freq + P.beta * (double)e;
-    inc = freq + P.alpha * (double)e;
-    phi = phi + inc;
-    freq = freq > P.fmax ? P.fmax : freq;
-    freq = freq < P.fmin ? P.fmin : freq;
+    freq = freq + P.beta * (double)e;                       // freq' (the clamp is the caller's, after it used freq')
+    phi = phi + freq + P.alpha * (double)e;
     phi = phi > two_pi ? phi - two_pi : phi;
     phi = phi < -two_pi ? phi + two_pi : phi;
     return e;
+}
+
+__device__ __forceinline__ void pll_clamp(double& freq, const PllParams& P) {
+    freq = freq > P.fmax ? P.fmax : freq;
+    freq = freq < P.fmin ? P.fmin : freq;
+}
+
+// phi_multiplied's step, as in pll_kernel
+__device__ __forceinline__ void pll_advance(double& phim, double freq, double e, const PllParams& P) {
+    const double two_pi = 6.283185307179586476925286766559;
+    phim = phim + freq * P.mult + P.alpha * e;
+    phim = phim > two_pi ? phim - two_pi : phim;
+    phim = phim < -two_pi ? phim + two_pi : phim;
 }
 
 __global__ void __launch_bounds__(128)
@@ -271,7 +283,7 @@ pll_sim_kernel(const float2* __restrict__ x, long long n, float* __restrict__ er
     const int c = blockIdx.x * blockDim.x + threadIdx.x;
     if (c >= nchunks) return;
     const long long start = (long long)c * L, end = start + L < n ? start + L : n;
-    double phi, freq, inc;
+    double phi, freq;
     if (c == 0) {
         phi = state[0];
         freq = state[2];
@@ -280,57 +292,54 @@ pll_sim_kernel(const float2* __restrict__ x, long long n, float* __restrict__ er
         const float2 x0 = x[begin];
         phi = (double)atan2f(x0.y, x0.x);
         freq = 0.5 * (P.fmin + P.fmax);
-        for (long long i = begin; i < start; ++i) pll_step(x[i], phi, freq, P, inc);
+        for (long long i = begin; i < start; ++i) {
+            pll_step(x[i], phi, freq, P);
+            pll_clamp(freq, P);
+        }
     }
     PllChunk r;
     r.freq0 = freq;
-    double dA = 0.0, dE = 0.0;
+    double dP = 0.0;
     for (long long i = start; i < end; ++i) {
-        const float e = pll_step(x[i], phi, freq, P, inc);
+        const float e = pll_step(x[i], phi, freq, P);
         err[i] = e;
-        dA += inc;
-        dE += (double)e;
+        pll_advance(dP, freq, (double)e, P);
+        pll_clamp(freq, P);
     }
-    r.dA = dA; r.dE = dE; r.phi_end = phi; r.freq_end = freq; r.A0 = 0.0; r.E0 = 0.0;
+    r.dP = dP; r.phi_end = phi; r.freq_end = freq; r.base = 0.0;
     chunks[c] = r;
 }
 
-__global__ void pll_prefix_kernel(PllChunk* chunks, int nchunks, double* state, PllParams P) {
+__global__ void pll_prefix_kernel(PllChunk* chunks, int nchunks, double* state) {
     if (blockIdx.x != 0 || threadIdx.x != 0) return;
     const double two_pi = 6.283185307179586476925286766559;
-    double A = 0.0, E = 0.0;
+    double ph = state[1];
     for (int c = 0; c < nchunks; ++c) {
-        chunks[c].A0 = A; chunks[c].E0 = E;
-        A += chunks[c].dA; E += chunks[c].dE;
+        chunks[c].base = ph;
+        ph = ph + chunks[c].dP;                              // |ph| <= 4 pi: one wrap brings it back, exactly
+        ph = ph > two_pi ? ph - two_pi : ph;
+        ph = ph < -two_pi ? ph + two_pi : ph;
     }
-    // carried state for the next call; state[3] keeps this call's phi_multiplied[0] for the output kernel
-    state[3] = state[1];
     state[0] = chunks[nchunks - 1].phi_end;
+    state[1] = ph;
     state[2] = chunks[nchunks - 1].freq_end;
-    state[1] = fmod(state[1] + P.mult * A + (1.0 - P.mult) * P.alpha * E, two_pi);
 }
 
 __global__ void __launch_bounds__(128)
 pll_out_kernel(const float* __restrict__ err, long long n, float2* __restrict__ out, long long L, int nchunks,
-               const double* __restrict__ state, PllParams P, const PllChunk* __restrict__ chunks) {
+               PllParams P, const PllChunk* __restrict__ chunks) {
     const int c = blockIdx.x * blockDim.x + threadIdx.x;
     if (c >= nchunks) return;
     const long long start = (long long)c * L, end = start + L < n ? start + L : n;
-    const double phim0 = state[3];
-    double A = chunks[c].A0, E = chunks[c].E0, freq = chunks[c].freq0;
-    const double two_pi = 6.283185307179586476925286766559;
+    double phim = chunks[c].base, freq = chunks[c].freq0;
     for (long long i = start; i < end; ++i) {
-        double ph = phim0 + P.mult * A + (1.0 - P.mult) * P.alpha * E;
-        ph -= two_pi * floor(ph / two_pi);                  // keep sincos in its accurate range
         double s, cc;
-        sincos(ph, &s, &cc);
+        sincos(phim, &s, &cc);
         out[i] = make_float2((float)cc, (float)s);
         const double e = (double)err[i];
         freq = freq + P.beta * e;
-        A += freq + P.alpha * e;
-        E += e;
-        freq = freq > P.fmax ? P.fmax : freq;
-        freq = freq < P.fmin ? P.fmin : freq;
+        pll_advance(phim, freq, e, P);
+        pll_clamp(freq, P);
     }
 }
 
@@ -340,7 +349,7 @@ pll_out_kernel(const float* __restrict__ err, long long n, float2* __restrict__ 
 struct PllBlock : Block {
     PllParams P;
     double init_freq;
-    DeviceBuffer d_state;           // phi_locked, phi_multiplied, freq_locked, (scratch) phi_multiplied at call start
+    DeviceBuffer d_state;           // phi_locked, phi_multiplied, freq_locked
     int mode = 0;                   // 0 = exact sequential, 1 = chunk-parallel (locked loop)
     long long warm = 0;             // lead-in of the chunk-parallel form
     DeviceBuffer d_chunks;
@@ -368,7 +377,7 @@ struct PllBlock : Block {
         LRB_CHECK(cudaStreamSynchronize(ctx().stream));
         return 0;
     }
-    int init() override { return d_state.reserve(4 * sizeof(double)) != 0 ? -1 : set_state(); }
+    int init() override { return d_state.reserve(3 * sizeof(double)) != 0 ? -1 : set_state(); }
     int reset() override { consumed = 0; return set_state(); }
     int run(const void*, size_t, void*, size_t*, cudaStream_t) override {
         set_error("pll has two outputs (out, error): use lrb200_block_execute_multi");
@@ -389,8 +398,8 @@ struct PllBlock : Block {
             PllChunk* chunks = d_chunks.as<PllChunk>();
             double* st = d_state.as<double>();
             pll_sim_kernel<<<blocks, 128, 0, s>>>((const float2*)dx[0], (long long)n, (float*)dy[1], L, warm, nchunks, st, P, chunks);
-            pll_prefix_kernel<<<1, 32, 0, s>>>(chunks, nchunks, st, P);
-            pll_out_kernel<<<blocks, 128, 0, s>>>((const float*)dy[1], (long long)n, (float2*)dy[0], L, nchunks, st, P, chunks);
+            pll_prefix_kernel<<<1, 32, 0, s>>>(chunks, nchunks, st);
+            pll_out_kernel<<<blocks, 128, 0, s>>>((const float*)dy[1], (long long)n, (float2*)dy[0], L, nchunks, P, chunks);
             count_launch(3);
             LRB_CHECK(cudaGetLastError());
             consumed += n;

@@ -222,6 +222,8 @@ def _general_iir_taps():
 HILBERT_TAPS = O.f32_taps(O.fir_hilbert_transform(33))
 PSD_FRAMES = (64, 1024)
 PLL_ARGS = (100.0, 19e3 - 50, 19e3 + 50, 2.0, 220500.0)
+PLL_L = 50536                      # aux_blocks.cu PllBlock: max(4 ceil(24 / (zeta bw)), 16384) for PLL_ARGS
+PLL_PARALLEL_LENGTHS = [1, 2 * PLL_L - 1, 2 * PLL_L, 2 * PLL_L + 1, 3 * PLL_L + 5]
 AGC_ARGS, AGC_RATE = ("custom", -20, -40, {"gain_tau": 1e-3, "power_tau": 5e-5}), 1e6
 SQ_ARGS, SQ_RATE = (-45,), 1e5
 
@@ -240,6 +242,20 @@ def _psd_case(N):
 def _pll_input(rng, n):
     t = np.arange(n) / PLL_ARGS[4]
     return [(0.8 * np.exp(2j * np.pi * 19000.3 * t + 0.4j) + 0.05 * rnd_c(rng, n)).astype(np.complex64)]
+
+
+def _pll_parallel(lib):
+    h = _lib.check_handle(lib.lrb200_pll_create(*PLL_ARGS, _lib.LRB200_DEVICE), "pll")
+    _lib.check(lib.lrb200_pll_set_mode(h, 1), "pll_set_mode")
+    return h
+
+
+def _pll_parallel_cmp():
+    from tests import pll_ref as P
+    lp = P.Loop(*PLL_ARGS)
+    assert lp.L == PLL_L
+    calls = PLL_PARALLEL_LENGTHS * len(_placements(1, 2))
+    return cmp_abs(2e-5 + max(P.ERR_TOL, P.out_tol(P.lead_ins(calls, lp))))
 
 
 def _level_case(agc, cplx):
@@ -353,6 +369,11 @@ BLOCK_CASES = {
     "pll": lambda: Case("lrb200_pll_create", lambda lib: lib.lrb200_pll_create(*PLL_ARGS, _lib.LRB200_DEVICE), [CPX], [CPX, FLT],
                         base_lengths(*EW_UNITS, big=3000), _pll_input,
                         lambda xs: list(O.PLL(*PLL_ARGS).process(xs[0])), cmp_abs(2e-5)),
+    # the chunk-parallel form (calls of 2 L and more; L = 50536 for these loop constants): ragged last chunks, the
+    # sequential form below 2 L in between.  Against the oracle at the sequential case's 2e-5 plus the parallel form's
+    # tolerance against the sequential one (tests/pll_ref.py)
+    "pll_parallel": lambda: Case("lrb200_pll_create", _pll_parallel, [CPX], [CPX, FLT], PLL_PARALLEL_LENGTHS, _pll_input,
+                                 lambda xs: list(O.PLL(*PLL_ARGS).process(xs[0])), _pll_parallel_cmp(), exact=True),
     **{"%s_%s" % ("agc" if agc else "powersquelch", "complex" if c else "real"): (lambda agc=agc, c=c: _level_case(agc, c))
        for agc in (True, False) for c in (False, True)},
     "phasecorrector_n50_i32": lambda: _phasecorr_case(50, 32),

@@ -362,8 +362,8 @@ def test_superchunk_scheduler_with_small_vectors():
 
 
 def test_pll_chunk_parallel_mode_when_locked():
-    """lrb200_pll_set_mode(1): every chunk simulated by its own thread after a lead-in, the multiplied phase rebuilt from
-    prefix sums.  Equal to the sequential recurrence while the loop is locked; the first chunk (carried state) is exact."""
+    """lrb200_pll_set_mode(1): every chunk simulated by its own thread after a lead-in, the multiplied phase carried
+    across the chunks as wrapped per-chunk advances.  Equal to the sequential recurrence while the loop is locked; the first chunk (carried state) is exact."""
     rate, n = 220500.0, 700000
     rng = np.random.default_rng(6)
     t = np.arange(n) / rate
@@ -389,5 +389,6 @@ def test_pll_chunk_parallel_mode_when_locked():
         close(got_e[:60000], re_[:60000], absolute=2e-5)            # sequential part: as test_pll_matches_the_restatement
         d_e = float(np.max(np.abs(got_e[60000:] - re_[60000:])))
         d_o = float(np.max(np.abs(got_o[60000:] - ref_out[60000:])))
-        assert d_e <= 2e-4 and d_o <= 2e-4, (multiplier, d_e, d_o)
+        print("multiplier %g: err %.3g, out %.3g" % (multiplier, d_e, d_o))
+        assert d_e <= 1e-6 and d_o <= 1e-6, (multiplier, d_e, d_o)        # 8.4e-8 on an H100
         blk.cleanup()

@@ -4,6 +4,7 @@
     the reference's 8192-sample vectors, give the same stream with `run(superchunk=S)` as with `run()`, for slots of whole
     vectors, of 2^20 samples, of a size no decimation divides, and smaller than one vector; the flush at end of stream
     drains a partial and an empty last slot, and a second run() of the same top block starts clean;
+  * the WBFM-stereo DAG in super-chunks with the chunk-parallel PLL equals the one with the serial PLL once locked;
   * lrb200_dag_execute_device returns bit for bit what lrb200_dag_execute returns for the same call lengths;
   * DEVICE-mode bounds: guard-banded, poisoned buffers at aligned and unaligned offsets (the harness of
     tests/test_gpu_bounds.py);
@@ -44,9 +45,12 @@ def stereo_input(n, seed):
     return (x * np.exp(2j * np.pi * 250e3 / RATE * np.arange(n))).astype(np.complex64)
 
 
-def stereo_top(x, chunk=VECTOR, src=None):
+def stereo_top(x, chunk=VECTOR, src=None, parallel_pll=False):
     src = src if src is not None else radio.ArraySource(x, RATE, chunk)
     demod, sinks = radio.WBFMStereoDemodulator(), [radio.ArraySink(), radio.ArraySink()]
+    for b in demod._blocks:
+        if isinstance(b, radio.PLLBlock):
+            b.parallel = parallel_pll
     top = radio.CompositeBlock()
     top.connect(src, radio.TunerBlock(-250e3, 200e3, 5), demod)
     top.connect(demod, "left", sinks[0], "in")
@@ -136,6 +140,28 @@ def test_superchunk_equals_streaming(name):
             assert len(g) == len(r) == len(e), "S=%d port %d: %d samples, streaming gave %d" % (S, k, len(g), len(r))
             assert np.array_equal(g.view(np.uint8), e.view(np.uint8)), "S=%d port %d differs from streaming in S-sample vectors" % (S, k)
             cmp(g, r, "S=%d port %d" % (S, k))
+
+
+@pytest.mark.parametrize("S", [1 << 20, 5 * (2 * 50536 + 1)])         # PLL calls of 5 chunks; of 2 L + 1 (a 1-sample chunk)
+def test_stereo_superchunk_with_the_chunk_parallel_pll(S):
+    """The WBFM-stereo DAG in super-chunks with PLLBlock.parallel = True against the same DAG with the serial PLL.  A
+    slot hands the PLL S / 5 samples, more than 2 L = 101072, so every call but the partial last one runs the
+    chunk-parallel form; its first chunk is exact and the loop has locked before the second chunk's lead-in starts.
+    Once locked (the lock index of cmp_stereo) the parallel PLL's output is within out_tol of tests/pll_ref.py of the
+    serial one, and the mixer, the two low-pass filters, Add / Subtract and the de-emphasis keep that
+    below 10 out_tol of the audio; before, both are held to the acquisition bound."""
+    from tests import pll_ref as P
+    x = stereo_input(N, 39)
+    _, serial = run_top(stereo_top, x, S)
+    top, par = run_top(lambda y: stereo_top(y, parallel_pll=True), x, S)
+    assert "pll" in top.describe_gpu_graph()
+    lock = 60000
+    for k, (g, r) in enumerate(zip(par, serial)):
+        assert len(g) == len(r) > lock
+        d = np.abs(g.astype(np.float64) - r)
+        print("port %d: parallel vs serial PLL %.3g before lock, %.3g after" % (k, float(d[:lock].max()), float(d[lock:].max())))
+        assert float(d[:lock].max()) <= 5e-3
+        assert float(d[lock:].max()) <= 10 * P.out_tol(-(-(N // 5) // 50536)), "port %d: locked: %.3g" % (k, float(d[lock:].max()))
 
 
 def test_superchunk_second_run_and_partial_last_slot():
