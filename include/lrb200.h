@@ -204,15 +204,23 @@ lrb200_block_t* lrb200_upsample_create(unsigned factor, unsigned elem_size, unsi
  * (loop_bandwidth, frequency_min, frequency_max) in Hz at `rate`, output 0 = exp(j phi_multiplied) (ComplexFloat32),
  * output 1 = phase error (Float32); execute through lrb200_block_execute_multi with one input and two outputs.  The
  * recurrence is nonlinear and is run in stream order by one thread (exact, a few MS/s).  lrb200_pll_set_mode(q, 1) opts
- * into the chunk-parallel form for long calls: each chunk is simulated by its own thread after a lead-in of
- * 24 / (zeta * loop bandwidth) samples from the phase of the input and the centre frequency; the multiplied phase is
- * carried across the chunks as per-chunk advances wrapped to +-2 pi at every step, as the sequential form wraps it, so
- * its rounding does not grow with the call.  It equals the sequential recurrence to the resolution of the float32 phase
- * detector WHILE THE LOOP IS LOCKED, not while it acquires or free-runs on noise. */
+ * into the chunk-parallel form for calls of 2 L samples or more (L = max(4 W, 16384), W = 24 / (zeta * loop bandwidth)):
+ * each chunk of L samples is simulated by its own thread after a W-sample lead-in from the phase of the input and the
+ * centre frequency.  One thread then checks every chunk's speculated start state against the true end state of the
+ * chunk before it, in stream order, and runs again, from the true state and with the sequential recurrence, every
+ * chunk that misses it by more than a threshold set from the loop constants.  The multiplied phase is carried across
+ * the chunks as per-chunk advances wrapped to +-2 pi at every step, as the sequential form wraps it, so its rounding
+ * does not grow with the call.  The result equals the sequential recurrence to the resolution of the float32 phase
+ * detector on any input, locked or not: where the loop is locked no chunk is run again and the call runs at the
+ * parallel rate; through zeros, noise or acquisition the chunks that miss cost one chunk of serial work each.
+ * lrb200_pll_chunk_counts synchronises the library stream and returns, since create or reset, the chunks run in the
+ * parallel form (each call's first chunk, which starts from the carried state, not counted) and how many of those were
+ * run again. */
 lrb200_block_t* lrb200_binary_create(const char* op, unsigned complex_data, unsigned flags);
 lrb200_block_t* lrb200_pll_create(double loop_bandwidth, double frequency_min, double frequency_max, double multiplier,
                                   double rate, unsigned flags);
 int lrb200_pll_set_mode(lrb200_block_t* q, int mode);
+int lrb200_pll_chunk_counts(lrb200_block_t* q, uint64_t* chunks, uint64_t* reruns);
 lrb200_block_t* lrb200_delay_create(unsigned num_samples, unsigned elem_size, unsigned flags);
 lrb200_block_t* lrb200_psd_create(unsigned num_samples, const float32_t* window, double scale, unsigned logarithmic,
                                   unsigned complex_data, unsigned flags);

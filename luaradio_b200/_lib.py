@@ -47,6 +47,7 @@ _PROTOS = {
     "lrb200_delay_create": (c_void_p, [c_uint, c_uint, c_uint]),
     "lrb200_pll_create": (c_void_p, [c_double, c_double, c_double, c_double, c_double, c_uint]),
     "lrb200_pll_set_mode": (c_int, [c_void_p, c_int]),
+    "lrb200_pll_chunk_counts": (c_int, [c_void_p, POINTER(c_uint64), POINTER(c_uint64)]),
     "lrb200_agc_create": (c_void_p, [c_double, c_double, c_double, c_double, c_double, c_uint, c_uint]),
     "lrb200_powersquelch_create": (c_void_p, [c_double, c_double, c_double, c_uint, c_uint]),
     "lrb200_phasecorrector_create": (c_void_p, [c_uint, c_uint, c_uint]),

@@ -455,7 +455,9 @@ class PLLBlock(GPUMultiBlock):
     """pll.lua:27-170: in -> out (exp(j * multiplied phase)), error (phase detector output)."""
     name = "PLLBlock"
 
-    parallel = False          # True: chunk-parallel form for long vectors (valid while the loop is locked; lrb200_pll_set_mode)
+    # True: chunk-parallel form for long vectors (lrb200_pll_set_mode(h, 1)); every chunk whose speculated start misses the
+    # carried loop state is run again in order, so it agrees with the sequential form on any input, locked or not
+    parallel = False
 
     def instantiate(self, loop_bandwidth, frequency_min, frequency_max, multiplier=None):
         assert loop_bandwidth is not None, "Missing argument #1 (loop_bandwidth)"
