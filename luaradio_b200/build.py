@@ -13,7 +13,7 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 BUILD = os.path.join(HERE, "_build")
 LIB = os.path.join(HERE, "libluaradio_b200.so")
-SOURCES = ["capi.cu", "graph.cu", "fir_direct.cu", "fir_fft.cu", "tuner.cu", "elementwise.cu", "iir.cu", "synth.cu", "iqconv.cu", "resample.cu", "aux_blocks.cu", "psd_long.cu", "poly_generic.cu", "level.cu", "phasecorr.cu", "iir_order.cu"]
+SOURCES = ["capi.cu", "graph.cu", "fir_direct.cu", "fir_fft.cu", "tuner.cu", "elementwise.cu", "iir.cu", "synth.cu", "iqconv.cu", "resample.cu", "aux_blocks.cu", "pll.cu", "psd_long.cu", "poly_generic.cu", "level.cu", "phasecorr.cu", "iir_order.cu"]
 NVCC = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
 # --split-compile 0: the fully unrolled tuner / FFT kernels are dozens of large kernels per file; let ptxas use every core.
 # With it the generated SASS depends on thread scheduling (two variants per file have been seen); LRB200_DETERMINISTIC=1 compiles single-threaded instead: reproducible, ~3x the build time.

@@ -1,6 +1,6 @@
-"""Float64 model, phase rebuild, per-output bound and deliberately wrong variants ("mutants") of PLLBlock's two GPU forms
-(aux_blocks.cu): the sequential kernel (pll_kernel) and the chunk-parallel one (pll_sim_kernel, pll_prefix_kernel,
-pll_out_kernel; lrb200_pll_set_mode(q, 1)).
+"""Float64 model, phase rebuild, per-output bound, acceptance thresholds and deliberately wrong variants ("mutants") of
+PLLBlock's two GPU forms (pll.cu): the sequential kernel (pll_kernel) and the verified chunk-parallel one
+(pll_sim_kernel, pll_verify_kernel, pll_out_kernel; lrb200_pll_set_mode(q, 1)).
 
 Recurrence (pll.lua:140-170, restated by oracle.lr_oracle.PLL).  Per sample, with e the float32 phase-detector output,
 
@@ -14,10 +14,20 @@ bw)) is the lead-in, L = max(4 W, 16384) the chunk length; chunk c covers [c L, 
 
   * sim: chunk 0 starts from the carried (phi, freq); every other chunk from phi = atan2f(x[c L - W]) and the centre
     frequency, run over the W samples before it (their errors are discarded).  Over its own samples each chunk writes e,
-    remembers freq0 (its frequency at its first sample) and sums its multiplied-phase advance dP with phim's own
-    expression, wrapped at every step.
+    remembers its speculated start (phi0, freq0: its state at its first sample), sums its multiplied-phase advance dP
+    with phim's own expression, wrapped at every step, and ends at (phi_end, freq_end).
+  * verify: the lead-in assumes that it reaches the loop's true trajectory.  It does not when the input gives the loop
+    nothing to pull with (zeros) or when the loop is not locked (noise, acquisition).  So each chunk's speculated start
+    is checked, in stream order, against the true state T:
+      - chunk 0: T is the carried state (chunk 0 starts from it, so it is always accepted);
+      - chunk c >= 1: T is chunk c - 1's (phi_end, freq_end), after any re-run of chunk c - 1.
+    Chunk c is accepted when |wrap(T.phi - phi0_c)| <= DPHI and |T.freq - freq0_c| <= DFREQ, the phase difference taken
+    modulo 2 pi (phi wraps at +-2 pi, and a lead-in that starts from atan2f lands on either branch).  Otherwise it is
+    re-run from T over its own samples with the sequential recurrence: err is rewritten, freq0 = T.freq, phi0 = T.phi
+    and dP, phi_end, freq_end are recomputed.  A re-run chunk is the sequential form's, bit for bit, whenever T is (so
+    err equals mode 0's on every sample before the first accepted chunk).
   * prefix: base_0 = the carried phim, base_{c+1} = wrap(base_c + dP_c); the carried state becomes the last chunk's
-    (phi, freq) and wrap(base_last + dP_last).
+    (phi_end, freq_end) and wrap(base_last + dP_last).
   * out: from (base_c, freq0_c) each chunk advances phim over its samples from the stored e, as the sequential form.
 
 Phase rebuild (`rebuild_phase`).  From a kernel's own e and the state at the start of the stream, freq' is recomputed
@@ -65,7 +75,50 @@ from the model against O.PLL, with 4x headroom or more:
 A lead-in of W / 2 still reaches the sequential trajectory on every input tried, including one whose phase guess is
 2.5 rad off (W is conservative), so no input here tells W / 2 from W: the lead-in mutant shortens it to W / 8, and the
 input that shows it turns the sample its phase guess is taken from.  The lead-in length is therefore checked only
-down to W / 8."""
+down to W / 8.
+
+Thresholds (`thresholds`).  Write a start-state offset (dphi, dfreq) against the true trajectory.  While the offset is
+small the float32 phase detector reads it as e' = e - dphi (atan2 of x conj(vco) turns with the VCO phase, whatever the
+amplitude), so the offsets follow the linearised loop
+
+    dfreq_{k+1} = dfreq_k - beta dphi_k
+    dphi_{k+1}  = dphi_k + dfreq_{k+1} - alpha dphi_k
+    dphim_{k+1} = dphim_k + m dfreq_{k+1} - alpha dphi_k          (dphim_0 = 0)
+
+(the clamp cannot widen a frequency difference).  The error differs by dphi_k and out by at most dphim_k, for the whole
+rest of the stream: a phase offset is never pulled back out of the multiplied phase (dphim tends to -m dphi_0 +
+(m - 1) alpha / beta dfreq_0).  `gains` iterates the system from (1, 0) and (0, 1) until both have died out and returns
+the largest |dphi_k| and |dphim_k| of each, G_e,phi, G_e,f, G_o,phi and G_o,f.  A chunk that starts exactly at the
+thresholds therefore leaves at most
+
+    |e - e_true|   <= G_e,phi DPHI + G_e,f DFREQ
+    |out - out_t|  <= G_o,phi DPHI + G_o,f DFREQ
+
+Two conditions are wanted: (a) every lead-in on a locked input accepted with a wide margin, so that locked input
+re-runs nothing, and (b) a chunk that starts exactly at the thresholds within the tolerances of the parallel form.
+The thresholds are a box (s alpha, s beta): the loop filter's step on one detector error s, the shape of what a lead-in
+leaves (it reaches the trajectory until a few float32 ulps of e, eps = 2^-23, tell them apart: the model observes at
+most 1.22 alpha eps and 0.57 beta eps over the inputs of test_pll_ref.py).  s is the largest that keeps a chunk
+starting at the box's corner within ERR_BUDGET = ERR_TOL / 4 in error and OUT_BUDGET = out_tol(1) - 2 OUT_ROUND =
+3.84e-7 in out (the two output roundings of any comparison are already in out_tol):
+
+    s = min(ERR_BUDGET / (G_e,phi alpha + G_e,f beta), OUT_BUDGET / (G_o,phi alpha + G_o,f beta))
+
+    loop      alpha    beta     DPHI     DFREQ     bound by   lead-in margin (phase, freq)
+    stereo    7.6e-3   2.9e-5   1.2e-7   4.4e-10   out        > 250x
+    rds       0.108    6.1e-3   7.1e-8   4.1e-9    out        ~10x, ~18x
+    am_sync   0.293    5.1e-2   1.8e-7   3.2e-8    error      >= 4x, >= 12x
+
+A lead-in that fails (zeros, noise, acquisition) misses by about the pilot's offset from the centre, 1e-5 rad/sample
+or more, and by radians in phase: orders of magnitude outside every box.
+
+Two limits of this choice.  (b) holds with 4x headroom for the error but only 1x for out: a 4x margin on out_tol(1)
+would put DPHI at 1e-8 for rds and 7e-8 for am_sync, inside what a converged lead-in leaves on a noisy pilot, and such
+a chunk would be run again for nothing.  And (a), 10x between the largest lead-in difference and the threshold, cannot
+hold for the am_sync loop together with (b): its worst lead-in (4.3e-8 rad on a noisy pilot) times 10 already moves
+out by 5.3e-7 > out_tol(1).  The tests assert 4x for (a) and ERR_TOL / 4 and out_tol(1) for (b).
+
+The GPU's PllBlock computes the same gains and thresholds in double (pll.cu, pll_thresholds)."""
 import math
 from fractions import Fraction
 
@@ -82,6 +135,8 @@ OUT_ROUND = math.sqrt(2.0) * 2.0 ** -25 + 1e-15
 MIN_CHUNK = 16384
 ERR_TOL = 1e-6
 OUT_TOL_CHUNK = 3.3e-8       # the model's worst out difference per sqrt(lead-in)
+ERR_BUDGET = 2.5e-7          # ERR_TOL / 4
+OUT_BUDGET = 3.84e-7         # out_tol(1) - 2 OUT_ROUND (3.849e-7), rounded down
 
 # (loop bandwidth, fmin, fmax, multiplier, rate): the receivers' loops
 LOOPS = {
@@ -89,14 +144,21 @@ LOOPS = {
     "rds": (1500.0, 19e3 - 100, 19e3 + 100, 3.0, 220500.0),        # the RDS receiver's baseband PLL
     "am_sync": (1000.0, 10e3 - 100, 10e3 + 100, 1.0, 48000.0),     # AMSynchronousDemodulator(10e3, ...) at 48 kS/s
 }
+# a carrier-recovery loop centred on 0 Hz: phi rotates slowly, so a lead-in's atan2f guess sits 2 pi from the true
+# branch on about half the chunks (what the wrap of the phase difference is for)
+BASEBAND = (1000.0, -100.0, 100.0, 1.0, 48000.0)
 
-MUTANTS = ("unreduced_prefix", "base_one_chunk_late", "phim0_after_call", "short_lead_in", "centre_freq_in_out_pass",
-           "no_e_term", "last_end_start_plus_L")
+MUTANTS = (
+    # the sim, prefix and out passes
+    "unreduced_prefix", "base_one_chunk_late", "phim0_after_call", "short_lead_in", "centre_freq_in_out_pass",
+    "no_e_term", "last_end_start_plus_L",
+    # the verify pass ("accept_all" is the unverified form: every lead-in accepted)
+    "accept_all", "rerun_from_speculated", "t_from_speculated_end", "stale_dP", "stale_freq0", "phase_without_wrap")
 A_OFFSET = 2.0 ** 26          # unreduced_prefix: the running sum A where a 2^27-sample call leaves it (0.5 rad/sample)
 
 
 class Loop:
-    """The loop constants of pll.lua:113-131 (as aux_blocks.cu PllBlock and O.PLL), the lead-in and the chunk length."""
+    """The loop constants of pll.lua:113-131 (as pll.cu PllBlock and O.PLL), the lead-in and the chunk length."""
 
     def __init__(self, bw_hz, fmin_hz, fmax_hz, mult, rate):
         o = O.PLL(bw_hz, fmin_hz, fmax_hz, mult, rate)
@@ -110,6 +172,49 @@ class Loop:
 
     def oracle(self):
         return O.PLL(*self.args)
+
+
+def loop(name, mult=None):
+    """The Loop of LOOPS[name] (or BASEBAND), with another multiplier if given."""
+    args = list(BASEBAND if name == "baseband" else LOOPS[name])
+    if mult is not None:
+        args[3] = mult
+    return Loop(*args)
+
+
+# ---- the thresholds -----------------------------------------------------------------------------------------------------
+def gains(loop, tail=1e-12):
+    """(G_e,phi, G_e,f, G_o,phi, G_o,f): the largest |dphi_k| and |dphim_k| of the linearised loop from a unit phase and
+    a unit frequency offset (see the module docstring).  Iterated until the state is below `tail` of its start."""
+    a, b, m = loop.alpha, loop.beta, loop.mult
+    res = []
+    for p, f in ((1.0, 0.0), (0.0, 1.0)):
+        pm, ge, go = 0.0, abs(p), 0.0
+        k = 0
+        while True:
+            f = f - b * p
+            pm = pm + m * f - a * p
+            p = p + f - a * p
+            ge, go = max(ge, abs(p)), max(go, abs(pm))
+            k += 1
+            if k > 64 and abs(p) < tail * ge and abs(f) < tail * b * ge:
+                break
+        res.append((ge, go))
+    (gep, gop), (gef, gof) = res
+    return gep, gef, gop, gof
+
+
+def thresholds(loop):
+    """(DPHI rad, DFREQ rad/sample) of the acceptance test (see the module docstring)."""
+    gep, gef, gop, gof = gains(loop)
+    a, b = loop.alpha, loop.beta
+    sc = min(ERR_BUDGET / (gep * a + gef * b), OUT_BUDGET / (gop * a + gof * b))
+    return sc * a, sc * b
+
+
+def wrap_diff(d):
+    """d reduced modulo 2 pi to [-pi, pi] (rint(d / 2 pi) turns, as the kernel)."""
+    return d - TWO_PI * np.rint(d / TWO_PI)
 
 
 # ---- the model --------------------------------------------------------------------------------------------------------
@@ -127,16 +232,21 @@ def _wrap(v):
 
 
 class Model:
-    """PLLBlock as the kernels compute it, call by call: mode 0 sequential, mode 1 chunk-parallel (n >= 2 L).
-    `process(x)` returns (out complex64, err float32); `mutant` selects one of MUTANTS."""
+    """PLLBlock as the kernels compute it, call by call: mode 0 sequential, mode 1 verified chunk-parallel (n >= 2 L).
+    `process(x)` returns (out complex64, err float32); `mutant` selects one of MUTANTS.  After each parallel call
+    `decisions` lists every chunk's (accepted, |phase difference|, |frequency difference|); `chunks` and `reruns` count
+    the speculated chunks (each call's chunks after the first) and how many of them were re-run since create or reset,
+    as lrb200_pll_chunk_counts."""
 
     def __init__(self, loop, mode=1, mutant=None):
         assert mutant is None or mutant in MUTANTS, mutant
         self.loop, self.mode, self.mutant = loop, mode, mutant
+        self.dphi, self.dfreq = thresholds(loop)
         self.reset()
 
     def reset(self):
         self.phi, self.phim, self.freq = 0.0, 0.0, self.loop.centre
+        self.chunks, self.reruns, self.decisions = 0, 0, []
 
     def process(self, x):
         x = np.asarray(x, np.complex64)
@@ -169,6 +279,15 @@ class Model:
         self.phi, self.phim, self.freq = phi, phim, freq
         return out, err
 
+    def _rerun(self, x, phi, freq):
+        """The chunk from (phi, freq) with the sequential recurrence: (err, dP, phi_end, freq_end)."""
+        keep = self.phi, self.phim, self.freq
+        self.phi, self.phim, self.freq = phi, 0.0, freq
+        _, err = self._sequential(x)
+        r = err, self.phim, self.phi, self.freq
+        self.phi, self.phim, self.freq = keep
+        return r
+
     def _parallel(self, x):
         lp, mut = self.loop, self.mutant
         n, L = len(x), lp.L
@@ -178,10 +297,18 @@ class Model:
         ends = np.minimum(starts + L, n)
         if mut == "last_end_start_plus_L":
             ends[-1] = starts[-1] + L                      # reads (zeros here) and runs past the call
+        span = int(np.max(ends - starts))
         xp = np.concatenate([x, np.zeros(int(ends[-1]) - n + 1, np.complex64)])
         xr, xi = xp.real.astype(F64), xp.imag.astype(F64)
         err = np.zeros(len(xp), F32)
-        # sim: lead-in of chunks 1.., then every chunk over its own samples
+
+        def advance(p, f, e):
+            # phi_multiplied's step (pll_advance), from freq' = f
+            if mut == "no_e_term":
+                return _wrap(p + (f + lp.alpha * e) * lp.mult)
+            return _wrap(p + f * lp.mult + lp.alpha * e)
+
+        # sim (pll_sim_kernel): the lead-ins of chunks 1.., then every chunk over its own samples
         phi = np.empty(nch)
         freq = np.full(nch, lp.centre)
         phi[0], freq[0] = self.phi, self.freq
@@ -193,25 +320,41 @@ class Model:
                 f = freq[1:] + lp.beta * e
                 phi[1:] = _wrap(phi[1:] + f + lp.alpha * e)
                 freq[1:] = np.clip(f, lp.fmin, lp.fmax)
-        freq0 = freq.copy()
-        dP, dA, dE = np.zeros(nch), np.zeros(nch), np.zeros(nch)
-        span = int(np.max(ends - starts))
+        phi0, freq0 = phi.copy(), freq.copy()
+        dP = np.zeros(nch)
         for t in range(span):
             act = starts + t < ends
             idx = np.where(act, starts + t, 0)
             e = _detect(xr[idx], xi[idx], phi)
             f = freq + lp.beta * e
-            ph_new = _wrap(phi + f + lp.alpha * e)
-            if mut == "no_e_term":
-                dP_new = _wrap(dP + (f + lp.alpha * e) * lp.mult)
-            else:
-                dP_new = _wrap(dP + f * lp.mult + lp.alpha * e)
             err[idx[act]] = e[act]
-            phi = np.where(act, ph_new, phi)
-            dP = np.where(act, dP_new, dP)
-            dA = np.where(act, dA + (f + lp.alpha * e), dA)
-            dE = np.where(act, dE + e, dE)
+            phi = np.where(act, _wrap(phi + f + lp.alpha * e), phi)
+            dP = np.where(act, advance(dP, f, e), dP)
             freq = np.where(act, np.clip(f, lp.fmin, lp.fmax), freq)
+        # verify (pll_verify_kernel), in stream order: phi, freq keep the speculated ends, phi_end, freq_end the true ones
+        phi_end, freq_end = phi.copy(), freq.copy()
+        self.decisions = []
+        Tphi, Tfreq = self.phi, self.freq
+        for c in range(nch):
+            if c > 0:
+                Tphi, Tfreq = (phi[c - 1], freq[c - 1]) if mut == "t_from_speculated_end" else (phi_end[c - 1], freq_end[c - 1])
+            d = Tphi - phi0[c]
+            dp = abs(d if mut == "phase_without_wrap" else float(wrap_diff(d)))
+            df = abs(Tfreq - freq0[c])
+            ok = mut == "accept_all" or (dp <= self.dphi and df <= self.dfreq)
+            self.decisions.append((ok, dp, df))
+            if ok:
+                continue
+            s, e_ = int(starts[c]), int(ends[c])
+            sphi, sfreq = (phi0[c], freq0[c]) if mut == "rerun_from_speculated" else (Tphi, Tfreq)
+            err[s:e_], dp_new, phi_end[c], freq_end[c] = self._rerun(xp[s:e_], sphi, sfreq)
+            if mut != "stale_dP":
+                dP[c] = dp_new
+            if mut != "stale_freq0":
+                freq0[c] = sfreq
+            phi0[c] = sphi
+        self.chunks += nch - 1
+        self.reruns += sum(not ok for ok, _, _ in self.decisions[1:])
         # prefix
         base = np.empty(nch)
         phim0 = self.phim
@@ -227,11 +370,17 @@ class Model:
             for c in range(nch):
                 base[c] = ph
                 ph = float(_wrap(np.array(ph + dP[c])))
+        # out (pll_out_kernel)
         out = np.zeros(len(xp), np.complex64)
         fr = np.full(nch, lp.centre) if mut == "centre_freq_in_out_pass" else freq0.copy()
         if mut == "unreduced_prefix":
-            # the earlier pll_out_kernel: phim0 + m A + (1 - m) alpha E from running sums A, E that start where a long
-            # call leaves them (A = A_OFFSET); the reference phase is then shifted by m A_OFFSET
+            # the earlier pll_out_kernel: phim0 + m A + (1 - m) alpha E from running sums A of freq' + alpha e and E of
+            # e that start where a long call leaves them (A = A_OFFSET); the reference phase is then shifted by m A_OFFSET
+            dA, dE = np.zeros(nch), np.zeros(nch)
+            for c in range(nch):
+                e = err[starts[c]:ends[c]].astype(F64)
+                dA[c] = np.add.accumulate(freq_prime(e, lp, freq0[c]) + lp.alpha * e)[-1]
+                dE[c] = np.add.accumulate(e)[-1]
             A0 = A_OFFSET + np.concatenate([[0.0], np.cumsum(dA)[:-1]])
             E0 = np.concatenate([[0.0], np.cumsum(dE)[:-1]])
             A, E = A0.copy(), E0.copy()
@@ -258,13 +407,9 @@ class Model:
                 out[idx[act]] = o[act]
                 e = err[idx].astype(F64)
                 f = fr + lp.beta * e
-                if mut == "no_e_term":
-                    pm_new = _wrap(pm + (f + lp.alpha * e) * lp.mult)
-                else:
-                    pm_new = _wrap(pm + f * lp.mult + lp.alpha * e)
-                pm = np.where(act, pm_new, pm)
+                pm = np.where(act, advance(pm, f, e), pm)
                 fr = np.where(act, np.clip(f, lp.fmin, lp.fmax), fr)
-        self.phi, self.phim, self.freq = float(phi[-1]), phim_end, float(freq[-1])
+        self.phi, self.phim, self.freq = float(phi_end[-1]), phim_end, float(freq_end[-1])
         return out[:n], err[:n]
 
 
@@ -443,3 +588,74 @@ def pilot(loop, n, kind="clean", amplitude=1.0, seed=0, t0=0):
     if kind == "noisy":
         x = x + amplitude * math.sqrt(0.1 / 2) * (rng.standard_normal(n) + 1j * rng.standard_normal(n))
     return x.astype(np.complex64)
+
+
+LOCKED = ("clean", "noisy", "offset", "drift")
+UNLOCKED = ("zeros_pilot", "gap", "noise_pilot", "pilot_noise_pilot", "zeros", "noise", "freq_step")
+
+
+def make_input(lp, kind, seed=21):
+    """(x, call lengths).  Locked pilots: a sequential acquisition call, then one parallel call of 4 L + 777.  The rest
+    run as one parallel call from a fresh loop: zeros (2.5 L) -> pilot; pilot (1.5 L) -> zeros -> pilot from W / 20
+    before chunk 4's boundary (its lead-in starts in the zeros and has not settled when the pilot is back); noise
+    (2 L) -> pilot; pilot -> noise (2 L) -> pilot; pure zeros and pure noise; a pilot that steps from +0.9 to -0.9 of
+    the half-range W / 10 before chunk 3's boundary, so that chunk's lead-in has not settled (6 L + 3 in all)."""
+    L = lp.L
+    if kind in LOCKED:
+        n1 = min(L, lp.W + 8000)
+        lengths = [n1, 4 * L + 777]
+        return pilot(lp, sum(lengths), kind, seed=seed), lengths
+    n = 6 * L + 3
+    if kind in ("zeros", "noise"):
+        return pilot(lp, n, kind, seed=seed), [n]
+    if kind == "freq_step":
+        bw, fmin, fmax, _, rate = lp.args
+        centre, half = 0.5 * (fmin + fmax), 0.5 * (fmax - fmin)
+        step = 3 * L - lp.W // 10
+        f = np.where(np.arange(n) < step, centre + 0.9 * half, centre - 0.9 * half)
+        ph = np.concatenate([[0.0], np.cumsum(2 * np.pi * f / rate)[:-1]])
+        return np.exp(1j * (np.mod(ph, 2 * np.pi) + 0.4)).astype(np.complex64), [n]
+    x = pilot(lp, n, "noisy", seed=seed)
+    gap, pos = (5 * L // 2 - lp.W // 20, 3 * L // 2) if kind == "gap" else (5 * L // 2, 0) if kind == "zeros_pilot" else (2 * L, 0) if kind == "noise_pilot" else (2 * L, 2 * L)
+    fill = np.zeros(gap, np.complex64) if kind in ("gap", "zeros_pilot") else pilot(lp, gap, "noise", seed=seed + 1)
+    x[pos:pos + gap] = fill
+    return x, [len(x)]
+
+
+def run_verified(lp, x, lengths, mutant=None):
+    """(out, err, model, decisions) of mode 1 over the calls; decisions: (first sample, accepted, |phase difference|,
+    |frequency difference|) of every speculated chunk."""
+    m = Model(lp, 1, mutant)
+    outs, errs, dec = [], [], []
+    pos = 0
+    for n in lengths:
+        o, e = m.process(x[pos:pos + n])
+        outs.append(o)
+        errs.append(e)
+        if n >= 2 * lp.L:
+            dec += [(pos + c * lp.L, ok, dp, df) for c, (ok, dp, df) in enumerate(m.decisions) if c > 0]
+        pos += n
+    return np.concatenate(outs), np.concatenate(errs), m, dec
+
+
+def check(lp, x, lengths, ref, got, locked):
+    """The assertions of the verified form, as a dict of name -> passed, plus the measured numbers: got = run_verified
+    (or the GPU's out and err with the model's decisions) against ref = mode 0's (out, err)."""
+    out, err, m, dec = got
+    accepted = [d for d in dec if d[1]]
+    tol = out_tol(len(accepted))
+    de = float(np.max(np.abs(err.astype(np.float64) - ref[1])))
+    do = float(np.max(np.abs(out.astype(np.complex128) - ref[0])))
+    first = accepted[0][0] if accepted else len(x)
+    res = {"err_tol": de <= ERR_TOL, "out_tol": do <= tol,
+           "err_exact_before_first_accept": bool(np.array_equal(err[:first], ref[1][:first]))}
+    nums = {"de": de / ERR_TOL, "do": do / tol, "accepted": len(accepted), "reruns": m.reruns, "chunks": m.chunks}
+    if locked:
+        res["no_reruns"] = m.reruns == 0
+        if accepted:
+            mp = max(d[2] for d in accepted) / m.dphi
+            mf = max(d[3] for d in accepted) / m.dfreq
+            nums["margin"] = 1.0 / max(mp, mf, 1e-300)
+            res["margin_a"] = nums["margin"] >= 4.0
+    print(nums, res)
+    return res, nums

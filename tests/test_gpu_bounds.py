@@ -222,7 +222,7 @@ def _general_iir_taps():
 HILBERT_TAPS = O.f32_taps(O.fir_hilbert_transform(33))
 PSD_FRAMES = (64, 1024)
 PLL_ARGS = (100.0, 19e3 - 50, 19e3 + 50, 2.0, 220500.0)
-PLL_L = 50536                      # aux_blocks.cu PllBlock: max(4 ceil(24 / (zeta bw)), 16384) for PLL_ARGS
+PLL_L = 50536                      # pll.cu PllBlock: max(4 ceil(24 / (zeta bw)), 16384) for PLL_ARGS
 PLL_PARALLEL_LENGTHS = [1, 2 * PLL_L - 1, 2 * PLL_L, 2 * PLL_L + 1, 3 * PLL_L + 5]
 AGC_ARGS, AGC_RATE = ("custom", -20, -40, {"gain_tau": 1e-3, "power_tau": 5e-5}), 1e6
 SQ_ARGS, SQ_RATE = (-45,), 1e5
