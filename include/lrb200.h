@@ -350,6 +350,45 @@ int    lrb200_dag_flush(lrb200_dag_t* d, void* const* y, size_t* n_out);
 int    lrb200_dag_reset(lrb200_dag_t* d);
 const char* lrb200_dag_describe(const lrb200_dag_t* d);
 void   lrb200_dag_destroy(lrb200_dag_t* d);
+/* Time-chunk sharding of a DAG (as lrb200_graph_halo / _execute_shard for linear graphs).  lrb200_dag_halo: input
+ * samples of left context a cold start needs -- walked back from the output ports, at a node's input ceil(max over its
+ * consumers of their need * down / up) + its memory + 1, a committed graph node by its own stages -- rounded up to 4 x
+ * the lcm of every output port's total decimation; < 0, with an error naming the block, when a node's memory is unbounded
+ * (AGC) or a PLL is behind another PLL.  A PLL counts as the lead-in of its chunk-parallel form (24 / (zeta * loop
+ * bandwidth) samples at its rate): its multiplied phase integrates the whole past, so it is handed from shard to shard at
+ * its HANDOFF POINT h, the PLL input index of a shard's start less what the nodes behind the PLL need of left context.
+ * lrb200_dag_seek seeks every node to the input index `sample_index` of the DAG input reaches it with.
+ *
+ * A shard runs chunk [start, start + n) from dx -> DEVICE [halo samples | n samples], cold from start - halo, and every
+ * port's outputs of the halo are dropped: dy[k] receives exactly the outputs of a single stream for the chunk.  start and
+ * halo are multiples of the period above and start >= halo (or start == 0 or halo == 0: the FIRST shard of a stream, which
+ * runs exactly lrb200_dag_execute_device after lrb200_dag_reset and lrb200_dag_seek(start)).  Not in super-chunk mode.
+ * Each PLL of the DAG contributes a record to an opaque blob of lrb200_dag_shard_record_bytes(d) bytes (0 for a DAG
+ * without a PLL; every call checks `record_bytes` against it): its speculated state at this shard's h, its state at the
+ * next shard's h, and the advance of its multiplied phase between the two.
+ *   1. lrb200_dag_shard_begin: resets the DAG, runs every node that is not behind a PLL (their ports' outputs go to dy),
+ *      runs each PLL's loop over its input speculated from h after a lead-in over the halo, and fills `record`: the one
+ *      synchronize.  n_out[k] is set for the ports it finished (every port of a DAG without a PLL: the shard is done)
+ *      and 0 for the rest.
+ *   2. Exchange: every shard's record reaches every shard to its right.
+ *   3. lrb200_dag_shard_accepts (host only): 1 when this shard's speculated start is within the PLL's acceptance
+ *      thresholds (those of the chunk-parallel form) of the left shard's end state for every PLL, else 0.
+ *   4. lrb200_dag_shard_end: left_records = the FINAL records of shards 0 .. r-1 (num_left = r, each blob in turn).  A
+ *      PLL whose start is not accepted runs its loop again from the left shard's end state; then each PLL's VCO output
+ *      starts from the multiplied phase the left shards' advances sum to, the nodes behind the PLLs run and every port's
+ *      kept outputs go to dy (n_out for every port).  record_out receives this shard's final record.  Returns 0 when every
+ *      PLL was accepted, 1 when one ran again (a synchronize more), -1 on error.
+ * Both PLL modes work (lrb200_pll_set_mode).  dx and the DAG stay in use until end returns; asynchronous on the library
+ * stream except for the record downloads.  A shard that runs again moves its end state: the shard to its right is tested
+ * against the new record (luaradio_b200/sharding.py, dag_shard_step). */
+long long lrb200_dag_halo(lrb200_dag_t* d);
+int    lrb200_dag_seek(lrb200_dag_t* d, uint64_t sample_index);
+size_t lrb200_dag_shard_record_bytes(lrb200_dag_t* d);
+int    lrb200_dag_shard_begin(lrb200_dag_t* d, const void* dx, size_t halo, size_t n, uint64_t start, void* const* dy,
+                              size_t* n_out, void* record, size_t record_bytes);
+int    lrb200_dag_shard_accepts(lrb200_dag_t* d, const void* left_record, const void* record, size_t record_bytes);
+int    lrb200_dag_shard_end(lrb200_dag_t* d, const void* left_records, unsigned num_left, void* const* dy, size_t* n_out,
+                            void* record_out, size_t record_bytes);
 
 /* ---- synthetic sources on the device (SURVEY.md 8d; the reference analogues are
  * radio/blocks/sources/{uniformrandom,signal}.lua) -- counter-based, so any window of the stream

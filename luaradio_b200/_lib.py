@@ -109,6 +109,12 @@ _PROTOS = {
     "lrb200_dag_set_superchunk": (c_int, [c_void_p, c_size_t]),
     "lrb200_dag_flush": (c_int, [c_void_p, POINTER(c_void_p), POINTER(c_size_t)]),
     "lrb200_dag_reset": (c_int, [c_void_p]),
+    "lrb200_dag_halo": (c_longlong, [c_void_p]),
+    "lrb200_dag_seek": (c_int, [c_void_p, c_uint64]),
+    "lrb200_dag_shard_record_bytes": (c_size_t, [c_void_p]),
+    "lrb200_dag_shard_begin": (c_int, [c_void_p, c_void_p, c_size_t, c_size_t, c_uint64, POINTER(c_void_p), POINTER(c_size_t), c_void_p, c_size_t]),
+    "lrb200_dag_shard_accepts": (c_int, [c_void_p, c_void_p, c_void_p, c_size_t]),
+    "lrb200_dag_shard_end": (c_int, [c_void_p, c_void_p, c_uint, POINTER(c_void_p), POINTER(c_size_t), c_void_p, c_size_t]),
     "lrb200_dag_describe": (c_char_p, [c_void_p]),
     "lrb200_dag_destroy": (None, [c_void_p]),
     "lrb200_synth_white_iq": (c_int, [c_void_p, c_uint64, c_size_t, c_uint32]),

@@ -312,6 +312,54 @@ struct PhaseCorrectorBlock : Block {
     long long memory_in() const override;
 };
 
+// pll.cu: PLLBlock.  Mode 0 runs the loop in stream order, mode 1 calls of 2 L samples or more in the verified
+// chunk-parallel form (pll.cu).  run_probe and the shard_* members are its part of a device DAG's time-chunk sharding
+// (graph.cu, Dag::shard_begin / shard_end).
+struct PllParams { double alpha, beta, fmin, fmax, mult; };
+struct PllBlock : Block {
+    PllParams P;
+    double init_freq;
+    DeviceBuffer d_state;           // phi_locked, phi_multiplied, freq_locked
+    int mode = 0;                   // 0 = exact sequential, 1 = chunk-parallel, verified against the carried state
+    long long warm = 0;             // lead-in of the chunk-parallel form
+    double dphi = 0.0, dfreq = 0.0; // acceptance thresholds of pll_verify_kernel
+    DeviceBuffer d_chunks;
+    DeviceBuffer d_reruns;          // chunks run again by pll_verify_kernel since create or reset
+    unsigned long long chunks_run = 0;  // chunks after the first of every parallel call since create or reset
+    // a shard's loop: the two ranges [lh, le) and [le, n) of its input, each run as a call of its length would run it
+    struct ShardRange { long long off = 0, len = 0, L = 1; int nch = 0, cb = 0; };   // cb: first chunk in d_chunks
+    ShardRange rng[2];
+    DeviceBuffer d_shard;           // (phi, sum of dP, freq) of the shard's loop
+
+    PllBlock(double loop_bw_hz, double fmin_hz, double fmax_hz, double multiplier, double rate, bool dev);
+    size_t out_size_of(int port) const override { return port == 0 ? 8 : 4; }
+    long long memory_in() const override { return -1; }        // the multiplied phase integrates the whole past
+    // the state after create and reset is not zero (freq_locked = init_freq): not carry()-declared
+    int set_state();
+    int init() override;
+    int reset() override { consumed = 0; return set_state(); }
+    int chunk_counts(uint64_t* chunks, uint64_t* reruns);
+    int run(const void*, size_t, void*, size_t*, cudaStream_t) override;
+    int run_multi(const void* const* dx, int nin, size_t n, void* const* dy, int nout, size_t* n_out, cudaStream_t s) override;
+    long long chunk_len() const { return warm * 4 > 16384 ? warm * 4 : 16384; }
+    bool parallel(size_t n) const { return mode == 1 && (long long)n >= 2 * chunk_len(); }
+    int reserve_chunks(int nchunks, cudaStream_t s);
+
+    // pll_accept on the host: is the speculated start (phi0, freq0) within (dphi, dfreq) of the true state?
+    bool accepts(double tphi, double tfreq, double phi0, double freq0) const;
+    // run_multi, and the state (phi, phim, freq) at sample split <= n of the call written to state_out (device)
+    int run_probe(const void* x, size_t n, void* const* dy, long long split, double* state_out, cudaStream_t s);
+    // errors of a shard's n input samples, the loop speculated from sample lh after the lead-in x[lh - warm, lh) (the
+    // errors before lh are zero); rec (device) receives {spec phi, spec freq, phi, sum of dP, freq}, the state at le and
+    // the advance of the multiplied phase over [lh, le) wrapped as pll_verify_kernel sums bases
+    int shard_loop(const void* x, size_t n, float* err, long long lh, long long le, double* rec, cudaStream_t s);
+    // the loop over [lh, n) again from the true state (tphi, tfreq) at lh; rewrites rec[2..5)
+    int shard_rerun(const void* x, float* err, double tphi, double tfreq, double* rec, cudaStream_t s);
+    // the VCO output of the shard from the multiplied phase `base` at lh (zeros before lh)
+    int shard_out(const float* err, float2* out, double base, cudaStream_t s);
+    int shard_range(const ShardRange& r, const void* x, float* err, bool rerun, cudaStream_t s);
+};
+
 // psd_long.cu: the PSD transform of frames of 8192 <= N <= 2^20 points (power of two) for PsdBlock
 constexpr int PSD_LONG_MIN = 8192, PSD_LONG_MAX = 1 << 20;
 constexpr int PSD_LONG_SINGLE_MAX = 16384;           // one CTA per frame up to here, two passes through scratch above

@@ -536,16 +536,24 @@ struct Graph : Block {
     }
     // input samples of left context a cold start needs so that the outputs equal the streaming ones to float32
     // resolution, rounded up to a whole number of output periods; < 0 when a stage's memory is unbounded
-    long long halo() {
+    // the input samples of left context that `need_out` outputs of left context need, unrounded (a Dag node's share of
+    // the DAG's halo); -1 with the error set when a stage's memory is unbounded
+    int need_in(double need_out, double* need) {
         if (ensure_committed() != 0) return -1;
-        double need = 0.0;                                   // at the input rate of the stage being visited
+        double nd = need_out;                                // at the input rate of the stage being visited
         for (size_t k = stages.size(); k-- > 0;) {
             unsigned bu, bd;
             stages[k]->rate(&bu, &bd);
             const long long mem = stages[k]->memory_in();
             if (mem < 0) { set_error("graph: %s has unbounded memory, the stream cannot be cut", stages[k]->name.c_str()); return -1; }
-            need = std::ceil(need * (double)bd / (double)bu) + (double)mem + 1.0;
+            nd = std::ceil(nd * (double)bd / (double)bu) + (double)mem + 1.0;
         }
+        *need = nd;
+        return 0;
+    }
+    long long halo() {
+        double need = 0.0;
+        if (need_in(0.0, &need) != 0) return -1;
         unsigned long long up, down;
         total_rate(&up, &down);
         // whole output periods, and a multiple of 4 samples so that a chunk placed `halo` samples into a 16-byte aligned
@@ -680,6 +688,7 @@ struct Dag {
         nd.out_buf.resize((size_t)blk->num_outputs);
         nd.out_cnt.assign((size_t)blk->num_outputs, 0);
         nd.out_ptr.assign((size_t)blk->num_outputs, nullptr);
+        sh.planned = false;
         if (!desc.empty()) desc += " ; ";
         desc += blk->name;
         nodes.push_back(std::move(nd));
@@ -731,41 +740,8 @@ struct Dag {
     // an edge buffer.
     int run_nodes(const void* dx, size_t n, void* const* dy, size_t* n_out, cudaStream_t s) {
         if (nodes.empty() || outputs.empty()) { set_error("dag: no nodes / no outputs"); return -1; }
-        for (size_t i = 0; i < nodes.size(); ++i) {
-            DagNode& nd = nodes[i];
-            std::vector<const void*> ins;
-            size_t cnt = 0;
-            for (size_t j = 0; j < nd.in_refs.size(); ++j) {
-                const int r = nd.in_refs[j];
-                const void* p = r == -1 ? dx : nodes[(size_t)(r >> 2)].out_ptr[(size_t)(r & 3)];
-                const size_t c = r == -1 ? n : nodes[(size_t)(r >> 2)].out_cnt[(size_t)(r & 3)];
-                if (j && c != cnt) { set_error("dag: %s received inputs of different lengths (%zu, %zu)", nd.blk->name.c_str(), cnt, c); return -1; }
-                cnt = c;
-                ins.push_back(p);
-            }
-            const int nout = nd.blk->num_outputs;
-            const size_t mo = nd.blk->max_output(cnt);
-            void* outs[4];                 // a port is two bits of a reference
-            for (int o = 0; o < nout; ++o) {
-                const int ref = (int)i * 4 + o;
-                void* ext = nullptr;
-                for (size_t k = 0; dy && k < outputs.size() && !ext; ++k)
-                    if (outputs[k] == ref) ext = dy[k];
-                if (!ext) {
-                    DeviceBuffer& buf = nd.out_buf[(size_t)o];
-                    const size_t bytes = (mo ? mo : 1) * nd.blk->out_size_of(o);
-                    if (bytes > buf.capacity()) {
-                        LRB_CHECK(cudaStreamSynchronize(s));
-                        if (buf.reserve(bytes) != 0) return -1;
-                    }
-                    ext = buf.get();
-                }
-                outs[o] = nd.out_ptr[(size_t)o] = ext;
-            }
-            size_t no = 0;
-            if (nd.blk->run_multi(ins.data(), (int)ins.size(), cnt, outs, nout, &no, s) != 0) return -1;
-            for (int o = 0; o < nout; ++o) nd.out_cnt[(size_t)o] = no;
-        }
+        for (size_t i = 0; i < nodes.size(); ++i)
+            if (run_node(i, dx, n, dy, s) != 0) return -1;
         for (size_t k = 0; k < outputs.size(); ++k) {
             const DagNode& nd = nodes[(size_t)(outputs[k] >> 2)];
             const size_t port = (size_t)(outputs[k] & 3), c = nd.out_cnt[port];
@@ -774,6 +750,60 @@ struct Dag {
                 LRB_CHECK(cudaMemcpyAsync(dy[k], nd.out_ptr[port], c * out_size(k), cudaMemcpyDeviceToDevice, s));
             n_out[k] = c;
         }
+        return 0;
+    }
+
+    // node i's inputs (all of the same length *cnt) and the places its ports write: a caller's dy[k] for output port k,
+    // else its grown edge buffer
+    int node_io(size_t i, const void* dx, size_t n, void* const* dy, std::vector<const void*>& ins, size_t* cnt, void** outs,
+                cudaStream_t s) {
+        DagNode& nd = nodes[i];
+        ins.clear();
+        *cnt = 0;
+        for (size_t j = 0; j < nd.in_refs.size(); ++j) {
+            const int r = nd.in_refs[j];
+            const void* p = r == -1 ? dx : nodes[(size_t)(r >> 2)].out_ptr[(size_t)(r & 3)];
+            const size_t c = r == -1 ? n : nodes[(size_t)(r >> 2)].out_cnt[(size_t)(r & 3)];
+            if (j && c != *cnt) { set_error("dag: %s received inputs of different lengths (%zu, %zu)", nd.blk->name.c_str(), *cnt, c); return -1; }
+            *cnt = c;
+            ins.push_back(p);
+        }
+        const size_t mo = nd.blk->max_output(*cnt);
+        for (int o = 0; o < nd.blk->num_outputs; ++o) {
+            const int ref = (int)i * 4 + o;
+            void* ext = nullptr;
+            for (size_t k = 0; dy && k < outputs.size() && !ext; ++k)
+                if (outputs[k] == ref) ext = dy[k];
+            if (!ext) {
+                DeviceBuffer& buf = nd.out_buf[(size_t)o];
+                const size_t bytes = (mo ? mo : 1) * nd.blk->out_size_of(o);
+                if (bytes > buf.capacity()) {
+                    LRB_CHECK(cudaStreamSynchronize(s));
+                    if (buf.reserve(bytes) != 0) return -1;
+                }
+                ext = buf.get();
+            }
+            outs[o] = nd.out_ptr[(size_t)o] = ext;
+        }
+        return 0;
+    }
+
+    // One node's launches.  A PLL with a probe point (sh.probe, the first rank of a sharded stream) also leaves its state
+    // there in its record.
+    int run_node(size_t i, const void* dx, size_t n, void* const* dy, cudaStream_t s) {
+        DagNode& nd = nodes[i];
+        std::vector<const void*> ins;
+        size_t cnt = 0;
+        void* outs[4];                 // a port is two bits of a reference
+        if (node_io(i, dx, n, dy, ins, &cnt, outs, s) != 0) return -1;
+        size_t no = 0;
+        if (!sh.probe.empty() && sh.probe[i] >= 0) {
+            if (static_cast<PllBlock*>(nd.blk.get())->run_probe(ins[0], cnt, outs, sh.probe[i], rec_dev(i) + 2, s) != 0) return -1;
+            no = cnt;
+        } else if (nd.blk->run_multi(ins.data(), (int)ins.size(), cnt, outs, nd.blk->num_outputs, &no, s) != 0) {
+            return -1;
+        }
+        for (int o = 0; o < nd.blk->num_outputs; ++o) nd.out_cnt[(size_t)o] = no;
         return 0;
     }
 
@@ -824,6 +854,285 @@ struct Dag {
         if (!sc_fed) { set_error("dag: nothing to flush: no execute since super-chunk mode was set, the last flush or reset"); return -1; }
         sc_fed = false;
         return sc.flush((char* const*)y, n_out, sc_run());
+    }
+
+    // ---- time-chunk sharding (SURVEY.md 8e) ---------------------------------------------------------------------------
+    // A shard runs the stream cold from start - halo and drops every port's outputs of the halo, as Graph::run_shard.  A
+    // PLL's multiplied phase integrates the whole past, so its state is handed over instead: at the PLL input index h of
+    // a shard's start, less what everything behind the PLL needs of left context (from h on, the PLL's outputs reach the
+    // shard's kept outputs), the loop is speculated from a lead-in over the halo (the chunk-parallel form's speculation,
+    // pll.cu), checked against the left shard's state at h, re-run from that state on a miss, and the VCO output is
+    // started from the sum of the left shards' advances of the multiplied phase.
+    static constexpr int REC = 6;    // doubles per PLL: spec phi, spec freq, end phi, end sum dP, end freq, first
+    struct ShardState {
+        std::vector<long long> probe;          // per node: the first shard's PLL probe point, or -1
+        std::vector<double> need_out;          // per node: outputs of left context its consumers and ports need
+        std::vector<char> below_pll;           // per node: a transitive consumer of a PLL
+        std::vector<int> pll_of;               // per node: index of its PLL record, or -1
+        std::vector<int> plls;                 // node ids of the PLLs
+        unsigned long long period = 1;         // lcm of every output port's total decimation
+        double need = 0.0;                     // input samples of left context, unrounded
+        // the shard between begin and end
+        bool pending = false, first = false;
+        const void* dx = nullptr;              // the DAG input (a PLL or a node behind one may read it)
+        uint64_t start = 0;
+        size_t halo = 0, n = 0;
+        std::vector<size_t> skip;              // per port: outputs of the halo
+        std::vector<double> rec;               // host copy of this shard's record
+        bool planned = false;
+    };
+    ShardState sh;
+    DeviceBuffer d_rec;
+    std::vector<double> h_rec;
+
+    double* rec_dev(size_t node) { return d_rec.as<double>() + (size_t)REC * (size_t)sh.pll_of[node]; }
+    size_t record_bytes() { return plan() != 0 ? 0 : sizeof(double) * REC * sh.plls.size(); }
+
+    // needs, PLLs and the period, from the shape alone; -1 with the error set when the stream cannot be cut
+    int plan() {
+        if (sh.planned) return 0;
+        if (nodes.empty() || outputs.empty()) { set_error("dag: no nodes / no outputs"); return -1; }
+        const size_t N = nodes.size();
+        sh.need_out.assign(N, 0.0);
+        sh.below_pll.assign(N, 0);
+        sh.pll_of.assign(N, -1);
+        sh.plls.clear();
+        std::vector<unsigned long long> up(N, 1), down(N, 1);        // total rate at each node's output
+        for (size_t i = 0; i < N; ++i) {
+            const DagNode& nd = nodes[i];
+            const bool pll = dynamic_cast<PllBlock*>(nd.blk.get()) != nullptr;
+            unsigned long long u = 1, d = 1;
+            for (int r : nd.in_refs)
+                if (r != -1) {
+                    const size_t p = (size_t)(r >> 2);
+                    if (sh.below_pll[p] || sh.pll_of[p] >= 0) sh.below_pll[i] = 1;
+                    u = up[p]; d = down[p];
+                }
+            if (pll && sh.below_pll[i]) { set_error("dag: %s behind another pll, the stream cannot be cut", nd.blk->name.c_str()); return -1; }
+            if (pll) { sh.pll_of[i] = (int)sh.plls.size(); sh.plls.push_back((int)i); }
+            unsigned bu, bd;
+            nd.blk->rate(&bu, &bd);
+            u *= bu; d *= bd;
+            unsigned long long a = u, c = d;
+            while (c) { const unsigned long long t = a % c; a = c; c = t; }
+            up[i] = u / a; down[i] = d / a;
+        }
+        sh.period = 1;
+        for (int r : outputs) {
+            const unsigned long long d = down[(size_t)(r >> 2)];
+            unsigned long long a = sh.period, c = d;
+            while (c) { const unsigned long long t = a % c; a = c; c = t; }
+            sh.period = sh.period / a * d;
+        }
+        // walk back from the ports: at a node's input, ceil(need at its output * down / up) + memory + 1
+        sh.need = 0.0;
+        for (size_t i = N; i-- > 0;) {
+            Block* b = nodes[i].blk.get();
+            double need;
+            if (Graph* g = dynamic_cast<Graph*>(b)) {
+                if (g->need_in(sh.need_out[i], &need) != 0) return -1;
+            } else if (PllBlock* p = dynamic_cast<PllBlock*>(b)) {
+                need = sh.need_out[i] + (double)p->warm + 1.0;     // the lead-in, behind the handoff point
+            } else {
+                const long long mem = b->memory_in();
+                if (mem < 0) { set_error("dag: %s has unbounded memory, the stream cannot be cut", b->name.c_str()); return -1; }
+                unsigned bu, bd;
+                b->rate(&bu, &bd);
+                need = std::ceil(sh.need_out[i] * (double)bd / (double)bu) + (double)mem + 1.0;
+            }
+            for (int r : nodes[i].in_refs) {
+                double& t = r == -1 ? sh.need : sh.need_out[(size_t)(r >> 2)];
+                t = need > t ? need : t;
+            }
+        }
+        sh.planned = true;
+        return 0;
+    }
+
+    long long halo() {
+        if (plan() != 0) return -1;
+        // whole output periods of every port, and a multiple of 4 samples so that a chunk placed `halo` samples into a
+        // 16-byte aligned buffer stays 16-byte aligned (as Graph::halo)
+        const long long q = 4 * (long long)sh.period;
+        const long long h = (long long)std::ceil(sh.need);
+        return ((h + q - 1) / q) * q;
+    }
+
+    // every node's input index once the DAG input's first `g` samples are consumed
+    std::vector<uint64_t> in_index(uint64_t g) const {
+        std::vector<uint64_t> idx(nodes.size());
+        for (size_t i = 0; i < nodes.size(); ++i) {
+            const int r = nodes[i].in_refs.empty() ? -1 : nodes[i].in_refs[0];
+            idx[i] = r == -1 ? g : nodes[(size_t)(r >> 2)].blk->outputs_before(idx[(size_t)(r >> 2)]);
+        }
+        return idx;
+    }
+
+    int seek(uint64_t g) {
+        const std::vector<uint64_t> idx = in_index(g);
+        for (size_t i = 0; i < nodes.size(); ++i)
+            if (nodes[i].blk->seek(idx[i]) != 0) return -1;
+        return 0;
+    }
+
+    int check_record(size_t bytes) {
+        const size_t want = record_bytes();
+        if (bytes != want) { set_error("dag: a record of this DAG is %zu bytes, got %zu", want, bytes); return -1; }
+        return 0;
+    }
+
+    // the kept outputs of port k (from its node's edge buffer) to dy[k]
+    int copy_port(size_t k, void* const* dy, size_t* n_out, cudaStream_t s) {
+        const DagNode& nd = nodes[(size_t)(outputs[k] >> 2)];
+        const size_t port = (size_t)(outputs[k] & 3), c = nd.out_cnt[port], sk = sh.skip[k];
+        if (c < sk) { set_error("dag: output %zu: the halo produced %zu outputs, expected %zu", k, c, sk); return -1; }
+        if (c > sk) LRB_CHECK(cudaMemcpyAsync(dy[k], (const char*)nd.out_ptr[port] + sk * out_size(k), (c - sk) * out_size(k),
+                                              cudaMemcpyDeviceToDevice, s));
+        n_out[k] = c - sk;
+        return 0;
+    }
+
+    bool port_in_phase_b(size_t k) const {
+        const size_t i = (size_t)(outputs[k] >> 2);
+        return sh.below_pll[i] || sh.pll_of[i] >= 0;
+    }
+
+    int shard_begin(const void* dx, size_t halo_n, size_t n, uint64_t start, void* const* dy, size_t* n_out, void* record,
+                    size_t record_bytes_) {
+        if (sc.samples) { set_error("dag: sharding runs the stream directly; switch super-chunk mode off first (set_superchunk 0)"); return -1; }
+        if (plan() != 0 || check_record(record_bytes_) != 0) return -1;
+        if (halo_n % sh.period || start % sh.period) { set_error("dag: halo and start must be multiples of %llu input samples", sh.period); return -1; }
+        const bool first = halo_n == 0 || start == 0;
+        if (!first && start < halo_n) { set_error("dag: chunk starts inside the halo"); return -1; }
+        sh.pending = false;
+        if (reset() != 0) return -1;
+        cudaStream_t s = ctx().stream;
+        const size_t npll = sh.plls.size();
+        if (npll && d_rec.reserve(sizeof(double) * REC * npll) != 0) return -1;
+        const uint64_t g0 = first ? start : start - halo_n;
+        if (seek(g0) != 0) return -1;
+        const std::vector<uint64_t> a0 = in_index(g0), a1 = in_index(start), a2 = in_index(start + n);
+        // handoff points of each PLL, as indices into this call's PLL input
+        std::vector<long long> lh(nodes.size(), -1), le(nodes.size(), -1);
+        for (int p : sh.plls) {
+            const long long D = (long long)std::ceil(sh.need_out[(size_t)p]);
+            lh[(size_t)p] = (long long)a1[(size_t)p] - D - (long long)a0[(size_t)p];
+            le[(size_t)p] = (long long)a2[(size_t)p] - D - (long long)a0[(size_t)p];
+            if (le[(size_t)p] < (first ? 0 : lh[(size_t)p])) { set_error("dag: the chunk is shorter than what follows %s needs", nodes[(size_t)p].blk->name.c_str()); return -1; }
+        }
+        sh.skip.assign(outputs.size(), 0);
+        int rc = 0;
+        if (first) {
+            // the plain run, with each PLL's state at the next shard's handoff point
+            sh.probe = le;
+            rc = run_nodes((const char*)dx + halo_n * in_size, n, dy, n_out, s);
+            sh.probe.clear();
+        } else {
+            for (size_t k = 0; k < outputs.size(); ++k) {
+                const size_t i = (size_t)(outputs[k] >> 2);
+                sh.skip[k] = (size_t)(nodes[i].blk->outputs_before(a1[i]) - nodes[i].blk->outputs_before(a0[i]));
+            }
+            const size_t N = halo_n + n;
+            for (size_t i = 0; i < nodes.size() && rc == 0; ++i) {
+                if (sh.below_pll[i]) continue;
+                if (sh.pll_of[i] < 0) { rc = run_node(i, dx, N, nullptr, s); continue; }
+                std::vector<const void*> ins;
+                size_t cnt = 0;
+                void* outs[4];
+                rc = node_io(i, dx, N, nullptr, ins, &cnt, outs, s);
+                if (rc == 0) rc = static_cast<PllBlock*>(nodes[i].blk.get())->shard_loop(ins[0], cnt, (float*)outs[1], lh[i], le[i], rec_dev(i), s);
+                nodes[i].out_cnt[0] = nodes[i].out_cnt[1] = cnt;
+            }
+            for (size_t k = 0; k < outputs.size() && rc == 0; ++k) {
+                n_out[k] = 0;
+                if (!port_in_phase_b(k)) rc = copy_port(k, dy, n_out, s);
+            }
+        }
+        if (rc != 0) return -1;
+        h_rec.assign(REC * npll, 0.0);
+        if (npll) {
+            LRB_CHECK(cudaMemcpyAsync(h_rec.data(), d_rec.get(), sizeof(double) * REC * npll, cudaMemcpyDeviceToHost, s));
+            LRB_CHECK(cudaStreamSynchronize(s));
+            for (size_t j = 0; j < npll; ++j) {
+                h_rec[REC * j + 5] = first ? 1.0 : 0.0;
+                if (first) h_rec[REC * j] = h_rec[REC * j + 1] = 0.0;     // no speculated start
+            }
+            memcpy(record, h_rec.data(), sizeof(double) * REC * npll);
+        }
+        sh.pending = true;
+        sh.first = first;
+        sh.start = start; sh.halo = halo_n; sh.n = n; sh.dx = dx;
+        return 0;
+    }
+
+    // does this shard's speculated start agree with the left shard's end state, for every PLL?
+    int shard_accepts(const double* left, const double* own) {
+        for (size_t j = 0; j < sh.plls.size(); ++j) {
+            const double* l = left + REC * j;
+            const double* o = own + REC * j;
+            if (o[5] != 0.0) continue;                               // a first shard starts from the reset state
+            const PllBlock* p = static_cast<const PllBlock*>(nodes[(size_t)sh.plls[j]].blk.get());
+            if (!p->accepts(l[2], l[4], o[0], o[1])) return 0;
+        }
+        return 1;
+    }
+
+    int shard_end(const double* left, unsigned num_left, void* const* dy, size_t* n_out, void* record_out, size_t record_bytes_) {
+        if (!sh.pending) { set_error("dag: shard_end without shard_begin"); return -1; }
+        if (check_record(record_bytes_) != 0) return -1;
+        const size_t npll = sh.plls.size();
+        cudaStream_t s = ctx().stream;
+        if (sh.first) {
+            for (size_t k = 0; k < outputs.size(); ++k) {
+                const DagNode& nd = nodes[(size_t)(outputs[k] >> 2)];
+                n_out[k] = nd.out_cnt[(size_t)(outputs[k] & 3)];
+            }
+            if (npll) memcpy(record_out, h_rec.data(), sizeof(double) * REC * npll);
+            sh.pending = false;
+            return 0;
+        }
+        if (npll && num_left == 0) { set_error("dag: a shard after the first needs the records of the shards to its left"); return -1; }
+        bool rerun = false;
+        int rc = 0;
+        for (size_t j = 0; j < npll && rc == 0; ++j) {
+            const size_t i = (size_t)sh.plls[j];
+            PllBlock* p = static_cast<PllBlock*>(nodes[i].blk.get());
+            const double* l = left + REC * npll * (size_t)(num_left - 1) + REC * j;
+            const double* o = h_rec.data() + REC * j;
+            // the multiplied phase at the handoff point: the left shards' advances, summed as pll_verify_kernel sums bases
+            double base = 0.0;
+            for (unsigned r = 0; r < num_left; ++r) {
+                base = base + left[(size_t)REC * (npll * r + j) + 3];
+                base = base > 6.283185307179586476925286766559 ? base - 6.283185307179586476925286766559 : base;
+                base = base < -6.283185307179586476925286766559 ? base + 6.283185307179586476925286766559 : base;
+            }
+            const int r = nodes[i].in_refs[0];
+            const void* x = r == -1 ? sh.dx : nodes[(size_t)(r >> 2)].out_ptr[(size_t)(r & 3)];
+            if (!p->accepts(l[2], l[4], o[0], o[1])) {
+                rerun = true;
+                rc = p->shard_rerun(x, (float*)nodes[i].out_ptr[1], l[2], l[4], rec_dev(i), s);
+            }
+            if (rc == 0) rc = p->shard_out((const float*)nodes[i].out_ptr[1], (float2*)nodes[i].out_ptr[0], base, s);
+        }
+        const size_t N = sh.halo + sh.n;
+        for (size_t i = 0; i < nodes.size() && rc == 0; ++i)
+            if (sh.below_pll[i]) rc = run_node(i, sh.dx, N, nullptr, s);
+        for (size_t k = 0; k < outputs.size() && rc == 0; ++k) {
+            if (port_in_phase_b(k)) rc = copy_port(k, dy, n_out, s);
+            else n_out[k] = nodes[(size_t)(outputs[k] >> 2)].out_cnt[(size_t)(outputs[k] & 3)] - sh.skip[k];
+        }
+        if (rc != 0) return -1;
+        if (rerun) {
+            // only the end states and sums are the device's: the speculated start and the first-shard flag stay the host's
+            std::vector<double> dev(REC * npll);
+            LRB_CHECK(cudaMemcpyAsync(dev.data(), d_rec.get(), sizeof(double) * REC * npll, cudaMemcpyDeviceToHost, s));
+            LRB_CHECK(cudaStreamSynchronize(s));
+            for (size_t j = 0; j < npll; ++j)
+                for (int f = 2; f < 5; ++f) h_rec[REC * j + f] = dev[REC * j + f];
+        }
+        if (npll) memcpy(record_out, h_rec.data(), sizeof(double) * REC * npll);
+        sh.pending = false;
+        return rerun ? 1 : 0;
     }
 };
 
@@ -1010,6 +1319,7 @@ int lrb200_dag_set_outputs(lrb200_dag_t* d, const int* outputs, unsigned num_out
         if (r < 0 || (r >> 2) >= (int)d->d.nodes.size() || (r & 3) >= d->d.nodes[(size_t)(r >> 2)].blk->num_outputs) { set_error("dag_set_outputs: bad reference %d", r); return -1; }
     }
     d->d.outputs.assign(outputs, outputs + num_outputs);
+    d->d.sh.planned = false;
     return 0;
 }
 
@@ -1043,6 +1353,37 @@ int lrb200_dag_flush(lrb200_dag_t* d, void* const* y, size_t* n_out) {
 int lrb200_dag_reset(lrb200_dag_t* d) {
     if (!d) { set_error("null dag"); return -1; }
     return d->d.reset();
+}
+
+long long lrb200_dag_halo(lrb200_dag_t* d) {
+    if (!d) { set_error("null dag"); return -1; }
+    return d->d.halo();
+}
+
+int lrb200_dag_seek(lrb200_dag_t* d, uint64_t sample_index) {
+    if (!d) { set_error("null dag"); return -1; }
+    if (d->d.nodes.empty()) { set_error("dag: no nodes"); return -1; }
+    return d->d.seek(sample_index);
+}
+
+size_t lrb200_dag_shard_record_bytes(lrb200_dag_t* d) { return d ? d->d.record_bytes() : 0; }
+
+int lrb200_dag_shard_begin(lrb200_dag_t* d, const void* dx, size_t halo, size_t n, uint64_t start, void* const* dy,
+                           size_t* n_out, void* record, size_t record_bytes) {
+    if (!d || !dy || !n_out || (n && !dx) || (record_bytes && !record)) { set_error("dag_shard_begin: null argument"); return -1; }
+    return d->d.shard_begin(dx, halo, n, start, dy, n_out, record, record_bytes);
+}
+
+int lrb200_dag_shard_accepts(lrb200_dag_t* d, const void* left_record, const void* record, size_t record_bytes) {
+    if (!d || (record_bytes && (!left_record || !record))) { set_error("dag_shard_accepts: null argument"); return -1; }
+    if (d->d.check_record(record_bytes) != 0) return -1;
+    return d->d.shard_accepts((const double*)left_record, (const double*)record);
+}
+
+int lrb200_dag_shard_end(lrb200_dag_t* d, const void* left_records, unsigned num_left, void* const* dy, size_t* n_out,
+                         void* record_out, size_t record_bytes) {
+    if (!d || !dy || !n_out || (record_bytes && (!record_out || (num_left && !left_records)))) { set_error("dag_shard_end: null argument"); return -1; }
+    return d->d.shard_end((const double*)left_records, num_left, dy, n_out, record_out, record_bytes);
 }
 
 const char* lrb200_dag_describe(const lrb200_dag_t* d) { return d ? d->d.desc.c_str() : ""; }

@@ -17,8 +17,6 @@ namespace {
 
 constexpr double PLL_TWO_PI = 6.283185307179586476925286766559;       // fl(2 pi): the wraps subtract it exactly
 
-struct PllParams { double alpha, beta, fmin, fmax, mult; };
-
 // The loop step on phi and freq: returns e and leaves phi updated and wrapped and freq = freq' (the clamp is the
 // caller's, after phi_multiplied's step has used freq').
 __device__ __forceinline__ float pll_step(float2 xv, double& phi, double& freq, const PllParams& P) {
@@ -230,92 +228,262 @@ void pll_thresholds(double alpha, double beta, double mult, double* dphi, double
     *dfreq = sc * beta;
 }
 
+
+// ---- time-chunk sharding of a device DAG (graph.cu, Dag::shard_begin / shard_end).  A shard's PLL input holds, before
+// the handoff point lh, a lead-in the left rank's samples fill; the loop is speculated from lh as pll_sim_kernel
+// speculates a chunk, and its state at lh, at the next rank's handoff point and the wrapped sum of the multiplied
+// phase's advances between them go to the shard's record: {spec phi, spec freq, end phi, end sum dP, end freq, first}.
+
+// the lead-in of pll_sim_kernel over x[lh - W, lh): st = (phi, 0, freq) and the record's speculated start
+__global__ void pll_lead_kernel(const float2* __restrict__ x, long long lh, long long W, PllParams P, double* st, double* rec) {
+    if (blockIdx.x != 0 || threadIdx.x != 0) return;
+    const float2 x0 = x[lh - W];
+    double phi = (double)atan2f(x0.y, x0.x), freq = 0.5 * (P.fmin + P.fmax);
+    for (long long i = lh - W; i < lh; ++i) {
+        pll_step(x[i], phi, freq, P);
+        pll_clamp(freq, P);
+    }
+    st[0] = phi; st[1] = 0.0; st[2] = freq;
+    rec[0] = phi; rec[1] = freq;
+}
+
+// one chunk of n samples in the sequential form from st, with its summary: what pll_verify_kernel makes of a re-run
+// chunk (st's phim is the chunk's base and advances by its dP, wrapped once)
+__global__ void pll_seq_kernel(const float2* __restrict__ x, long long n, float* __restrict__ err, double* st, PllParams P,
+                               PllChunk* chunk) {
+    if (blockIdx.x != 0 || threadIdx.x != 0) return;
+    PllChunk k = pll_chunk(x, err, 0, n, st[0], st[2], P);
+    k.base = st[1];
+    double ph = st[1] + k.dP;
+    ph = ph > PLL_TWO_PI ? ph - PLL_TWO_PI : ph;
+    ph = ph < -PLL_TWO_PI ? ph + PLL_TWO_PI : ph;
+    st[0] = k.phi_end; st[1] = ph; st[2] = k.freq_end;
+    *chunk = k;
+}
+
+// the bases of nchunks consecutive chunks from base0, summed as pll_verify_kernel sums them
+__global__ void pll_rebase_kernel(PllChunk* chunks, int nchunks, double base0) {
+    if (blockIdx.x != 0 || threadIdx.x != 0) return;
+    double ph = base0;
+    for (int c = 0; c < nchunks; ++c) {
+        chunks[c].base = ph;
+        ph = ph + chunks[c].dP;
+        ph = ph > PLL_TWO_PI ? ph - PLL_TWO_PI : ph;
+        ph = ph < -PLL_TWO_PI ? ph + PLL_TWO_PI : ph;
+    }
+}
+
+// after a chunk-parallel call: the loop state (phi, phim, freq) at sample `split` <= n, replayed from the start state of
+// the chunk that holds it -- the state its errors were computed from -- and its base
+__global__ void pll_probe_kernel(const float2* __restrict__ x, long long L, const PllChunk* __restrict__ chunks, int nchunks,
+                                 long long split, PllParams P, double* out) {
+    if (blockIdx.x != 0 || threadIdx.x != 0) return;
+    int c = (int)(split / L);
+    c = c < nchunks - 1 ? c : nchunks - 1;
+    double phi = chunks[c].phi0, freq = chunks[c].freq0, phim = chunks[c].base;
+    for (long long i = (long long)c * L; i < split; ++i) {
+        const float e = pll_step(x[i], phi, freq, P);
+        pll_advance(phim, freq, (double)e, P);
+        pll_clamp(freq, P);
+    }
+    out[0] = phi; out[1] = phim; out[2] = freq;
+}
+
 }  // namespace
 
-struct PllBlock : Block {
-    PllParams P;
-    double init_freq;
-    DeviceBuffer d_state;           // phi_locked, phi_multiplied, freq_locked
-    int mode = 0;                   // 0 = exact sequential, 1 = chunk-parallel, verified against the carried state
-    long long warm = 0;             // lead-in of the chunk-parallel form
-    double dphi = 0.0, dfreq = 0.0; // acceptance thresholds of pll_verify_kernel
-    DeviceBuffer d_chunks;
-    DeviceBuffer d_reruns;          // chunks run again by pll_verify_kernel since create or reset
-    unsigned long long chunks_run = 0;  // chunks after the first of every parallel call since create or reset
-    PllBlock(double loop_bw_hz, double fmin_hz, double fmax_hz, double multiplier, double rate, bool dev) : Block("pll", 8, 8, dev) {
-        num_outputs = 2;
-        // pll.lua:113-131
-        double bw = 2 * M_PI * (loop_bw_hz / rate);
-        P.fmin = 2 * M_PI * (fmin_hz / rate);
-        P.fmax = 2 * M_PI * (fmax_hz / rate);
-        const double damping = std::sqrt(2.0) / 2;
-        bw = bw / (damping + 1 / (4 * damping));
-        const double denom = 1 + 2 * damping * bw + bw * bw;
-        P.alpha = (4 * damping * bw) / denom;
-        P.beta = (4 * bw * bw) / denom;
-        P.mult = multiplier;
-        init_freq = (P.fmin + P.fmax) / 2.0;
-        warm = (long long)std::ceil(24.0 / (damping * bw));
-        pll_thresholds(P.alpha, P.beta, P.mult, &dphi, &dfreq);
+PllBlock::PllBlock(double loop_bw_hz, double fmin_hz, double fmax_hz, double multiplier, double rate, bool dev) : Block("pll", 8, 8, dev) {
+    num_outputs = 2;
+    // pll.lua:113-131
+    double bw = 2 * M_PI * (loop_bw_hz / rate);
+    P.fmin = 2 * M_PI * (fmin_hz / rate);
+    P.fmax = 2 * M_PI * (fmax_hz / rate);
+    const double damping = std::sqrt(2.0) / 2;
+    bw = bw / (damping + 1 / (4 * damping));
+    const double denom = 1 + 2 * damping * bw + bw * bw;
+    P.alpha = (4 * damping * bw) / denom;
+    P.beta = (4 * bw * bw) / denom;
+    P.mult = multiplier;
+    init_freq = (P.fmin + P.fmax) / 2.0;
+    warm = (long long)std::ceil(24.0 / (damping * bw));
+    pll_thresholds(P.alpha, P.beta, P.mult, &dphi, &dfreq);
+}
+
+int PllBlock::set_state() {
+    const double h[3] = {0.0, 0.0, init_freq};
+    LRB_CHECK(cudaMemcpyAsync(d_state.get(), h, sizeof(h), cudaMemcpyHostToDevice, ctx().stream));
+    LRB_CHECK(cudaMemsetAsync(d_reruns.get(), 0, sizeof(unsigned long long), ctx().stream));
+    LRB_CHECK(cudaStreamSynchronize(ctx().stream));
+    chunks_run = 0;
+    return 0;
+}
+
+int PllBlock::init() {
+    return d_state.reserve(3 * sizeof(double)) != 0 || d_reruns.reserve(sizeof(unsigned long long)) != 0 ||
+                   d_shard.reserve(3 * sizeof(double)) != 0
+               ? -1
+               : set_state();
+}
+
+int PllBlock::chunk_counts(uint64_t* chunks, uint64_t* reruns) {
+    unsigned long long r = 0;
+    LRB_CHECK(cudaMemcpyAsync(&r, d_reruns.get(), sizeof(r), cudaMemcpyDeviceToHost, ctx().stream));
+    LRB_CHECK(cudaStreamSynchronize(ctx().stream));
+    if (chunks) *chunks = chunks_run;
+    if (reruns) *reruns = r;
+    return 0;
+}
+
+int PllBlock::run(const void*, size_t, void*, size_t*, cudaStream_t) {
+    set_error("pll has two outputs (out, error): use lrb200_block_execute_multi");
+    return -1;
+}
+
+int PllBlock::reserve_chunks(int nchunks, cudaStream_t s) {
+    if (sizeof(PllChunk) * (size_t)nchunks > d_chunks.capacity()) {
+        LRB_CHECK(cudaStreamSynchronize(s));
+        if (d_chunks.reserve(sizeof(PllChunk) * (size_t)nchunks) != 0) return -1;
     }
-    size_t out_size_of(int port) const override { return port == 0 ? 8 : 4; }
-    long long memory_in() const override { return -1; }        // the multiplied phase integrates the whole past
-    // the state after create and reset is not zero (freq_locked = init_freq): not carry()-declared
-    int set_state() {
-        const double h[3] = {0.0, 0.0, init_freq};
-        LRB_CHECK(cudaMemcpyAsync(d_state.get(), h, sizeof(h), cudaMemcpyHostToDevice, ctx().stream));
-        LRB_CHECK(cudaMemsetAsync(d_reruns.get(), 0, sizeof(unsigned long long), ctx().stream));
-        LRB_CHECK(cudaStreamSynchronize(ctx().stream));
-        chunks_run = 0;
-        return 0;
-    }
-    int init() override {
-        return d_state.reserve(3 * sizeof(double)) != 0 || d_reruns.reserve(sizeof(unsigned long long)) != 0 ? -1 : set_state();
-    }
-    int reset() override { consumed = 0; return set_state(); }
-    int chunk_counts(uint64_t* chunks, uint64_t* reruns) {
-        unsigned long long r = 0;
-        LRB_CHECK(cudaMemcpyAsync(&r, d_reruns.get(), sizeof(r), cudaMemcpyDeviceToHost, ctx().stream));
-        LRB_CHECK(cudaStreamSynchronize(ctx().stream));
-        if (chunks) *chunks = chunks_run;
-        if (reruns) *reruns = r;
-        return 0;
-    }
-    int run(const void*, size_t, void*, size_t*, cudaStream_t) override {
-        set_error("pll has two outputs (out, error): use lrb200_block_execute_multi");
-        return -1;
-    }
-    int run_multi(const void* const* dx, int nin, size_t n, void* const* dy, int nout, size_t* n_out, cudaStream_t s) override {
-        if (nin != 1 || nout != 2) { set_error("pll: expected 1 input and 2 outputs"); return -1; }
-        *n_out = n;
-        if (n == 0) return 0;
-        const long long L = warm * 4 > 16384 ? warm * 4 : 16384;
-        if (mode == 1 && (long long)n >= 2 * L) {
-            const int nchunks = (int)(((long long)n + L - 1) / L);
-            if (sizeof(PllChunk) * (size_t)nchunks > d_chunks.capacity()) {
-                LRB_CHECK(cudaStreamSynchronize(s));
-                if (d_chunks.reserve(sizeof(PllChunk) * (size_t)nchunks) != 0) return -1;
-            }
-            const int blocks = (nchunks + 127) / 128;
-            PllChunk* chunks = d_chunks.as<PllChunk>();
-            double* st = d_state.as<double>();
-            pll_sim_kernel<<<blocks, 128, 0, s>>>((const float2*)dx[0], (long long)n, (float*)dy[1], L, warm, nchunks, st, P, chunks);
-            pll_verify_kernel<<<1, PV_BATCH, 0, s>>>((const float2*)dx[0], (long long)n, (float*)dy[1], L, chunks, nchunks, st, P,
-                                                     dphi, dfreq, d_reruns.as<unsigned long long>());
-            pll_out_kernel<<<blocks, 128, 0, s>>>((const float*)dy[1], (long long)n, (float2*)dy[0], L, nchunks, P, chunks);
-            count_launch(3);
-            LRB_CHECK(cudaGetLastError());
-            chunks_run += (unsigned long long)(nchunks - 1);
-            consumed += n;
-            return 0;
-        }
-        pll_kernel<<<1, 32, 0, s>>>((const float2*)dx[0], (long long)n, (float2*)dy[0], (float*)dy[1], d_state.as<double>(), P);
-        count_launch();
+    return 0;
+}
+
+int PllBlock::run_multi(const void* const* dx, int nin, size_t n, void* const* dy, int nout, size_t* n_out, cudaStream_t s) {
+    if (nin != 1 || nout != 2) { set_error("pll: expected 1 input and 2 outputs"); return -1; }
+    *n_out = n;
+    if (n == 0) return 0;
+    const long long L = chunk_len();
+    if (parallel(n)) {
+        const int nchunks = (int)(((long long)n + L - 1) / L);
+        if (reserve_chunks(nchunks, s) != 0) return -1;
+        const int blocks = (nchunks + 127) / 128;
+        PllChunk* chunks = d_chunks.as<PllChunk>();
+        double* st = d_state.as<double>();
+        pll_sim_kernel<<<blocks, 128, 0, s>>>((const float2*)dx[0], (long long)n, (float*)dy[1], L, warm, nchunks, st, P, chunks);
+        pll_verify_kernel<<<1, PV_BATCH, 0, s>>>((const float2*)dx[0], (long long)n, (float*)dy[1], L, chunks, nchunks, st, P,
+                                                 dphi, dfreq, d_reruns.as<unsigned long long>());
+        pll_out_kernel<<<blocks, 128, 0, s>>>((const float*)dy[1], (long long)n, (float2*)dy[0], L, nchunks, P, chunks);
+        count_launch(3);
         LRB_CHECK(cudaGetLastError());
+        chunks_run += (unsigned long long)(nchunks - 1);
         consumed += n;
         return 0;
     }
-};
+    pll_kernel<<<1, 32, 0, s>>>((const float2*)dx[0], (long long)n, (float2*)dy[0], (float*)dy[1], d_state.as<double>(), P);
+    count_launch();
+    LRB_CHECK(cudaGetLastError());
+    consumed += n;
+    return 0;
+}
+
+// ---- time-chunk sharding of a device DAG --------------------------------------------------------------------------------
+bool PllBlock::accepts(double tphi, double tfreq, double phi0, double freq0) const {
+    double d = tphi - phi0;                            // pll_accept, on the host
+    d = d - PLL_TWO_PI * std::rint(d / PLL_TWO_PI);
+    return std::fabs(d) <= dphi && std::fabs(tfreq - freq0) <= dfreq;
+}
+
+int PllBlock::run_probe(const void* x, size_t n, void* const* dy, long long split, double* state_out, cudaStream_t s) {
+    if (split < 0 || split > (long long)n) { set_error("pll: probe at %lld outside a call of %zu samples", split, n); return -1; }
+    size_t no = 0;
+    if (parallel(n)) {
+        if (run_multi(&x, 1, n, dy, 2, &no, s) != 0) return -1;
+        const long long L = chunk_len();
+        pll_probe_kernel<<<1, 32, 0, s>>>((const float2*)x, L, d_chunks.as<PllChunk>(), (int)(((long long)n + L - 1) / L), split, P,
+                                          state_out);
+        count_launch();
+        LRB_CHECK(cudaGetLastError());
+        return 0;
+    }
+    // the sequential form carries its whole state from call to call: two calls split at `split` are the one call bit for bit
+    double* st = d_state.as<double>();
+    if (split > 0) {
+        pll_kernel<<<1, 32, 0, s>>>((const float2*)x, split, (float2*)dy[0], (float*)dy[1], st, P);
+        count_launch();
+    }
+    LRB_CHECK(cudaMemcpyAsync(state_out, st, 3 * sizeof(double), cudaMemcpyDeviceToDevice, s));
+    if ((long long)n > split) {
+        pll_kernel<<<1, 32, 0, s>>>((const float2*)x + split, (long long)n - split, (float2*)dy[0] + split, (float*)dy[1] + split, st, P);
+        count_launch();
+    }
+    LRB_CHECK(cudaGetLastError());
+    consumed += n;
+    return 0;
+}
+
+// the loop over x[off, off + len) from d_shard in the form a call of len samples runs (rerun: the chunks were simulated
+// before, and are verified again against a new d_shard)
+int PllBlock::shard_range(const ShardRange& r, const void* x, float* err, bool rerun, cudaStream_t s) {
+    if (r.len == 0) return 0;
+    const float2* xr = (const float2*)x + r.off;
+    PllChunk* chunks = d_chunks.as<PllChunk>() + r.cb;
+    double* st = d_shard.as<double>();
+    if (r.nch == 1) {
+        pll_seq_kernel<<<1, 32, 0, s>>>(xr, r.len, err + r.off, st, P, chunks);
+        count_launch();
+    } else {
+        if (!rerun) {
+            pll_sim_kernel<<<(r.nch + 127) / 128, 128, 0, s>>>(xr, r.len, err + r.off, r.L, warm, r.nch, st, P, chunks);
+            chunks_run += (unsigned long long)(r.nch - 1);
+            count_launch();
+        }
+        pll_verify_kernel<<<1, PV_BATCH, 0, s>>>(xr, r.len, err + r.off, r.L, chunks, r.nch, st, P, dphi, dfreq,
+                                                 d_reruns.as<unsigned long long>());
+        count_launch();
+    }
+    LRB_CHECK(cudaGetLastError());
+    return 0;
+}
+
+int PllBlock::shard_loop(const void* x, size_t n, float* err, long long lh, long long le, double* rec, cudaStream_t s) {
+    if (lh < warm || le < lh || le > (long long)n) {
+        set_error("pll: handoff points %lld, %lld of a %zu-sample shard leave no %lld-sample lead-in", lh, le, n, warm);
+        return -1;
+    }
+    const long long L = chunk_len();
+    const long long off[3] = {lh, le, (long long)n};
+    int cb = 0;
+    for (int k = 0; k < 2; ++k) {
+        ShardRange& r = rng[k];
+        r.off = off[k];
+        r.len = off[k + 1] - off[k];
+        r.L = parallel((size_t)r.len) ? L : (r.len > 0 ? r.len : 1);
+        r.nch = r.len == 0 ? 0 : (int)((r.len + r.L - 1) / r.L);
+        r.cb = cb;
+        cb += r.nch;
+    }
+    if (reserve_chunks(cb > 0 ? cb : 1, s) != 0) return -1;
+    if (lh > 0) LRB_CHECK(cudaMemsetAsync(err, 0, (size_t)lh * sizeof(float), s));
+    pll_lead_kernel<<<1, 32, 0, s>>>((const float2*)x, lh, warm, P, d_shard.as<double>(), rec);
+    count_launch();
+    if (shard_range(rng[0], x, err, false, s) != 0) return -1;
+    LRB_CHECK(cudaMemcpyAsync(rec + 2, d_shard.get(), 3 * sizeof(double), cudaMemcpyDeviceToDevice, s));
+    if (shard_range(rng[1], x, err, false, s) != 0) return -1;
+    consumed += n;
+    return 0;
+}
+
+int PllBlock::shard_rerun(const void* x, float* err, double tphi, double tfreq, double* rec, cudaStream_t s) {
+    const double h[3] = {tphi, 0.0, tfreq};
+    LRB_CHECK(cudaMemcpyAsync(d_shard.get(), h, sizeof(h), cudaMemcpyHostToDevice, s));
+    if (shard_range(rng[0], x, err, true, s) != 0) return -1;
+    LRB_CHECK(cudaMemcpyAsync(rec + 2, d_shard.get(), 3 * sizeof(double), cudaMemcpyDeviceToDevice, s));
+    return shard_range(rng[1], x, err, true, s);
+}
+
+int PllBlock::shard_out(const float* err, float2* out, double base, cudaStream_t s) {
+    const int nch = rng[0].nch + rng[1].nch;
+    if (rng[0].off > 0) LRB_CHECK(cudaMemsetAsync(out, 0, (size_t)rng[0].off * sizeof(float2), s));
+    if (nch == 0) return 0;
+    PllChunk* chunks = d_chunks.as<PllChunk>();
+    pll_rebase_kernel<<<1, 32, 0, s>>>(chunks, nch, base);
+    count_launch();
+    for (const ShardRange& r : rng) {
+        if (r.nch == 0) continue;
+        pll_out_kernel<<<(r.nch + 127) / 128, 128, 0, s>>>(err + r.off, r.len, out + r.off, r.L, r.nch, P, chunks + r.cb);
+        count_launch();
+    }
+    LRB_CHECK(cudaGetLastError());
+    return 0;
+}
 
 }  // namespace lrb
 

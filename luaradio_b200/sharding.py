@@ -61,3 +61,68 @@ def trim_outputs(n_out_total, lead, total_decimation):
     assert lead % total_decimation == 0
     skip = lead // total_decimation
     return skip, n_out_total - skip
+
+
+def dag_shard_step(dist, lib, dag, dx, halo, n, start, dy, n_out, rank, world, device="cpu", times=None):
+    """One step of a sharded device DAG (lrb200_dag_shard_*, include/lrb200.h) on every rank: dx -> [halo | n] input
+    samples on this rank's device, chunk starting at `start`; dy / n_out as lrb200_dag_shard_end takes them (ctypes
+    arrays).  Returns 1 when this rank's PLL ran again, else 0.
+
+    1. every rank begins: the nodes that are not behind a PLL run, and each PLL's loop from its speculated start;
+    2. the records (a few dozen bytes each) are all-gathered;
+    3. k = the first rank whose start its left neighbour's record does not accept;
+    4. ranks below k end with the gathered records;
+    5. from k on, each rank ends with the final records of the ranks to its left, received from its left neighbour, and
+       passes them on with its own: a rank that ran again moves its end state, so its right neighbour is tested again.
+    A step with no miss costs the one all-gather.  Records travel as float64 tensors on `device` (the backend's).  A dict
+    `times` receives the seconds of begin, of the exchange (begin's return to end's call) and of end."""
+    import ctypes
+    import time
+    import torch
+    t0 = time.perf_counter()
+    nb = lib.lrb200_dag_shard_record_bytes(dag)
+    rec = (ctypes.c_double * max(1, nb // 8))()
+    ptr = lambda a: ctypes.cast(a, ctypes.c_void_p)
+    rc = lib.lrb200_dag_shard_begin(dag, dx, halo, n, start, dy, n_out, ptr(rec), nb)
+    if rc != 0:
+        raise RuntimeError("dag_shard_begin: rc %d" % rc)
+    t1 = time.perf_counter()
+    if times is not None:
+        times.update(begin=t1 - t0, exchange=0.0, end=0.0)
+    if nb == 0:
+        return 0
+    m = nb // 8
+    mine = torch.tensor(list(rec)[:m], dtype=torch.float64, device=device)
+    gathered = [torch.empty(m, dtype=torch.float64, device=device) for _ in range(world)]
+    dist.all_gather(gathered, mine)
+    recs = [g.cpu().numpy() for g in gathered]
+
+    def carr(rows):
+        flat = [float(v) for r in rows for v in r]
+        return (ctypes.c_double * max(1, len(flat)))(*flat)
+
+    k = world
+    for j in range(1, world):
+        a = lib.lrb200_dag_shard_accepts(dag, ptr(carr([recs[j - 1]])), ptr(carr([recs[j]])), nb)
+        if a < 0:
+            raise RuntimeError("dag_shard_accepts failed")
+        if a == 0:
+            k = j
+            break
+    lefts = recs[:rank]
+    if rank > k:
+        buf = torch.empty(rank * m, dtype=torch.float64, device=device)
+        dist.recv(buf, rank - 1)
+        flat = buf.cpu().numpy()
+        lefts = [flat[i * m:(i + 1) * m] for i in range(rank)]
+    out = (ctypes.c_double * m)()
+    t2 = time.perf_counter()
+    rc = lib.lrb200_dag_shard_end(dag, ptr(carr(lefts)), rank, dy, n_out, ptr(out), nb)
+    if times is not None:
+        times.update(exchange=t2 - t1, end=time.perf_counter() - t2)
+    if rc < 0:
+        raise RuntimeError("dag_shard_end: rc %d" % rc)
+    if rank >= k and rank + 1 < world:
+        final = [list(r) for r in lefts] + [list(out)]
+        dist.send(torch.tensor([v for r in final for v in r], dtype=torch.float64, device=device), rank + 1)
+    return rc
