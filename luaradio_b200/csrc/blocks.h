@@ -5,11 +5,15 @@
 #include <cmath>
 #include <memory>
 #include <new>
+#include <numeric>
+#include <type_traits>
 #include <vector>
 #include <string>
 #include <utility>
 
 namespace lrb {
+
+struct PllBlock;
 
 struct Block {
     std::string name;
@@ -51,6 +55,11 @@ struct Block {
     virtual long long memory_in() const { return 0; }
     // output rate / input rate = up / down
     virtual void rate(unsigned* up, unsigned* down) const { *up = 1; *down = 1; }
+    // the input samples of left context that `need_out` outputs of left context need, unrounded: ceil(need_out * down /
+    // up) + memory_in() + 1.  -1 with the error set when the memory is unbounded (the stream cannot be cut here).
+    virtual int need_in(double need_out, double* need) const;
+    // this block as a PLL whose loop state a sharded DAG hands from shard to shard, else null
+    virtual PllBlock* as_pll() { return nullptr; }
     // sharded runs: can this block's launch keep the launches that read the first Ctx::lead_samples inputs behind
     // Ctx::lead_event while everything else starts at once?  (else the whole stream waits for the neighbour exchange)
     virtual bool supports_lead_wait() const { return false; }
@@ -58,6 +67,17 @@ struct Block {
     // stream for a long call (edge tiles, history update)?  Then a short call may run entirely on the side stream and the
     // next long call's interior kernel need not wait for it (run_shard's split of the last stage).
     virtual bool state_only_on_side_stream() const { return false; }
+};
+
+// A rate change in lowest terms: outputs per input = up / down
+struct Rate {
+    unsigned long long up = 1, down = 1;
+    Rate then(const Block& b) const {       // this rate followed by b's
+        unsigned bu, bd;
+        b.rate(&bu, &bd);
+        const unsigned long long u = up * bu, d = down * bd, g = std::gcd(u, d);
+        return Rate{u / g, d / g};
+    }
 };
 
 // Construct and init() a block: nullptr, with the error set, on failure
@@ -316,6 +336,11 @@ struct PhaseCorrectorBlock : Block {
 // chunk-parallel form (pll.cu).  run_probe and the shard_* members are its part of a device DAG's time-chunk sharding
 // (graph.cu, Dag::shard_begin / shard_end).
 struct PllParams { double alpha, beta, fmin, fmax, mult; };
+// One PLL's part of a DAG shard's record (lrb200_dag_shard_*): the loop state speculated at the shard's handoff point,
+// the state at the next shard's handoff point and the wrapped sum of the multiplied phase's advances between the two,
+// and 1 for the stream's first shard (which speculates nothing).  Its bytes are the record's: the callers exchange them.
+struct PllShardRecord { double spec_phi, spec_freq, end_phi, end_dP, end_freq, first; };
+static_assert(sizeof(PllShardRecord) == 48 && std::is_standard_layout<PllShardRecord>::value, "six doubles, in this order");
 struct PllBlock : Block {
     PllParams P;
     double init_freq;
@@ -334,6 +359,9 @@ struct PllBlock : Block {
     PllBlock(double loop_bw_hz, double fmin_hz, double fmax_hz, double multiplier, double rate, bool dev);
     size_t out_size_of(int port) const override { return port == 0 ? 8 : 4; }
     long long memory_in() const override { return -1; }        // the multiplied phase integrates the whole past
+    // in a DAG the loop's state is handed over instead: the lead-in, behind the handoff point
+    int need_in(double need_out, double* need) const override { *need = need_out + (double)warm + 1.0; return 0; }
+    PllBlock* as_pll() override { return this; }
     // the state after create and reset is not zero (freq_locked = init_freq): not carry()-declared
     int set_state();
     int init() override;
@@ -347,14 +375,17 @@ struct PllBlock : Block {
 
     // pll_accept on the host: is the speculated start (phi0, freq0) within (dphi, dfreq) of the true state?
     bool accepts(double tphi, double tfreq, double phi0, double freq0) const;
-    // run_multi, and the state (phi, phim, freq) at sample split <= n of the call written to state_out (device)
-    int run_probe(const void* x, size_t n, void* const* dy, long long split, double* state_out, cudaStream_t s);
+    // the multiplied phase at a shard's handoff point: the end_dP of the left shards' records (num_left records of
+    // `stride` PLLs each, this PLL's at index j), summed and wrapped as pll_verify_kernel sums bases
+    static double fold_advances(const PllShardRecord* lefts, unsigned num_left, size_t stride, size_t j);
+    // run_multi, and the state (phi, phim, freq) at sample split <= n of the call written to rec's end state (device)
+    int run_probe(const void* x, size_t n, void* const* dy, long long split, PllShardRecord* rec, cudaStream_t s);
     // errors of a shard's n input samples, the loop speculated from sample lh after the lead-in x[lh - warm, lh) (the
-    // errors before lh are zero); rec (device) receives {spec phi, spec freq, phi, sum of dP, freq}, the state at le and
+    // errors before lh are zero); rec (device) receives the speculated start, and as its end state the state at le and
     // the advance of the multiplied phase over [lh, le) wrapped as pll_verify_kernel sums bases
-    int shard_loop(const void* x, size_t n, float* err, long long lh, long long le, double* rec, cudaStream_t s);
-    // the loop over [lh, n) again from the true state (tphi, tfreq) at lh; rewrites rec[2..5)
-    int shard_rerun(const void* x, float* err, double tphi, double tfreq, double* rec, cudaStream_t s);
+    int shard_loop(const void* x, size_t n, float* err, long long lh, long long le, PllShardRecord* rec, cudaStream_t s);
+    // the loop over [lh, n) again from the true state (tphi, tfreq) at lh; rewrites rec's end state
+    int shard_rerun(const void* x, float* err, double tphi, double tfreq, PllShardRecord* rec, cudaStream_t s);
     // the VCO output of the shard from the multiplied phase `base` at lh (zeros before lh)
     int shard_out(const float* err, float2* out, double base, cudaStream_t s);
     int shard_range(const ShardRange& r, const void* x, float* err, bool rerun, cudaStream_t s);

@@ -291,6 +291,34 @@ struct SuperChunk {
     size_t max_output(size_t k, size_t n) const { return (n / samples + 2) * outcap[k]; }
 };
 
+// ---- time-chunk sharding (SURVEY.md 8e): where a stream can be cut, for graphs and DAGs alike ---------------------------
+int Block::need_in(double need_out, double* need) const {
+    const long long mem = memory_in();
+    if (mem < 0) { set_error("%s has unbounded memory, the stream cannot be cut", name.c_str()); return -1; }
+    unsigned bu, bd;
+    rate(&bu, &bd);
+    *need = std::ceil(need_out * (double)bd / (double)bu) + (double)mem + 1.0;
+    return 0;
+}
+
+// The halo of a left-context need: whole output periods, and a multiple of 4 samples so that a chunk placed `halo`
+// samples into a 16-byte aligned buffer stays 16-byte aligned (float32 and complex streams alike): the vectorised interior
+// kernels need that.  `need` is a whole number (need_in adds whole numbers to a ceil), so the ceil only converts it.
+static long long round_halo(double need, unsigned long long period) {
+    const long long q = 4 * (long long)period;
+    const long long h = (long long)std::ceil(need);
+    return ((h + q - 1) / q) * q;
+}
+
+// The arguments of one shard of a stream whose output period is `period` input samples: 0 with *first set for the
+// stream's first chunk (no halo, or start 0: nothing to its left), or -1 with the error set
+static int shard_args(const char* who, size_t halo, uint64_t start, unsigned long long period, bool* first) {
+    if (halo % period || start % period) { set_error("%s: halo and start must be multiples of %llu input samples", who, period); return -1; }
+    *first = halo == 0 || start == 0;
+    if (!*first && start < halo) { set_error("%s: chunk starts inside the halo", who); return -1; }
+    return 0;
+}
+
 // A committed linear run of blocks, itself a one-port Block (a node of a Dag).  Its name is the description.
 struct Graph : Block {
     Blocks blocks;                   // as appended
@@ -350,9 +378,8 @@ struct Graph : Block {
         return idx;
     }
     void rate(unsigned* up, unsigned* down) const override {
-        unsigned long long u, d;
-        total_rate(&u, &d);
-        *up = (unsigned)u; *down = (unsigned)d;
+        const Rate r = total_rate();
+        *up = (unsigned)r.up; *down = (unsigned)r.down;
     }
 
     int commit(int fuse) {
@@ -521,47 +548,24 @@ struct Graph : Block {
     int reset() override { return reset(ctx().stream); }
 
     // ---- time-chunk sharding (SURVEY.md 8e) -------------------------------------------------------------------
-    // total rate change in lowest terms: outputs per input = up / down
-    void total_rate(unsigned long long* up, unsigned long long* down) const {
-        unsigned long long u = 1, d = 1;
-        for (Block* b : stages) {
-            unsigned bu, bd;
-            b->rate(&bu, &bd);
-            u *= bu; d *= bd;
-            unsigned long long a = u, c = d;
-            while (c) { unsigned long long t = a % c; a = c; c = t; }
-            u /= a; d /= a;
-        }
-        *up = u; *down = d;
+    Rate total_rate() const {
+        Rate r;
+        for (Block* b : stages) r = r.then(*b);
+        return r;
     }
-    // input samples of left context a cold start needs so that the outputs equal the streaming ones to float32
-    // resolution, rounded up to a whole number of output periods; < 0 when a stage's memory is unbounded
-    // the input samples of left context that `need_out` outputs of left context need, unrounded (a Dag node's share of
-    // the DAG's halo); -1 with the error set when a stage's memory is unbounded
-    int need_in(double need_out, double* need) {
-        if (ensure_committed() != 0) return -1;
-        double nd = need_out;                                // at the input rate of the stage being visited
-        for (size_t k = stages.size(); k-- > 0;) {
-            unsigned bu, bd;
-            stages[k]->rate(&bu, &bd);
-            const long long mem = stages[k]->memory_in();
-            if (mem < 0) { set_error("graph: %s has unbounded memory, the stream cannot be cut", stages[k]->name.c_str()); return -1; }
-            nd = std::ceil(nd * (double)bd / (double)bu) + (double)mem + 1.0;
-        }
-        *need = nd;
+    // the stages walked back from the output, each by the plain rule (a PLL's state is handed over only in a DAG)
+    int need_in(double need_out, double* need) const override {
+        for (size_t k = stages.size(); k-- > 0;)
+            if (stages[k]->Block::need_in(need_out, &need_out) != 0) return -1;
+        *need = need_out;
         return 0;
     }
+    // input samples of left context a cold start needs so that the outputs equal the streaming ones to float32
+    // resolution, as a halo; -1 when a stage's memory is unbounded
     long long halo() {
         double need = 0.0;
-        if (need_in(0.0, &need) != 0) return -1;
-        unsigned long long up, down;
-        total_rate(&up, &down);
-        // whole output periods, and a multiple of 4 samples so that a chunk placed `halo` samples into a 16-byte aligned
-        // buffer stays 16-byte aligned (float32 and complex streams alike): the vectorised interior kernels need that
-        const long long q = 4 * (long long)down;
-        long long h = (long long)need;
-        h = ((h + q - 1) / q) * q;
-        return h;
+        if (ensure_committed() != 0 || need_in(0.0, &need) != 0) return -1;
+        return round_halo(need, total_rate().down);
     }
 
     // One time chunk of a sharded stream.  dx -> [halo samples of the left neighbour | n samples of this chunk], the chunk
@@ -578,14 +582,12 @@ struct Graph : Block {
         if (stages.empty()) { set_error("graph: no blocks"); return -1; }
         cudaStream_t s = ctx().stream;
         const size_t isz = in_size, osz = out_size;
-        unsigned long long up, down;
-        total_rate(&up, &down);
-        if (halo_n % down || start % down) { set_error("graph: halo and start must be multiples of %llu input samples", down); return -1; }
-        if (halo_n == 0 || start == 0) {                     // the stream's first chunk: nothing to its left
+        bool first;
+        if (shard_args("graph", halo_n, start, total_rate().down, &first) != 0) return -1;
+        if (first) {
             if (reset(s) != 0 || seek(start) != 0) return -1;
             return run((const char*)dx + halo_n * isz, n, dy, n_out, s);
         }
-        if (start < halo_n) { set_error("graph: chunk starts inside the halo"); return -1; }
         if (reset(s) != 0 || seek(start - halo_n) != 0) return -1;
         const size_t K = stages.size();
         // inputs of every stage that belong to the halo: lead[k] = (stage-k input index of `start`) - (that of start - halo)
@@ -663,17 +665,29 @@ struct Graph : Block {
 // device-resident input and outputs with no synchronize; or host vectors packed into super-chunks (SuperChunk above).
 // This is what composites/wbfmstereodemodulator.lua:22-64 and amsynchronousdemodulator.lua:25-45 need on the device.
 // ---------------------------------------------------------------------------------------------------------------------
+// An output port of a node, or (node -1) the DAG's input.  The C ABI encodes it as node * 4 + port, or -1.
+struct PortRef {
+    int node = -1, port = 0;
+    bool is_input() const { return node < 0; }
+};
+
 struct DagNode {
     std::unique_ptr<Block> blk;    // a block, or a committed linear Graph
-    std::vector<int> in_refs;      // producer node * 4 + port, or -1 for the DAG input
+    std::vector<PortRef> ins;
     std::vector<DeviceBuffer> out_buf;
     std::vector<size_t> out_cnt;
     std::vector<void*> out_ptr;    // where each port's samples of the current call are (out_buf, or a caller's dy)
+    // time-chunk sharding, from the DAG's shape (Dag::plan)
+    double need_out = 0.0;         // outputs of left context its consumers and ports need
+    bool below_pll = false;        // a transitive consumer of a PLL
+    PllBlock* pll = nullptr;       // the block as a PLL whose state is handed over (set by add), with its record's index
+    int rec = -1;
+    long long probe = -1;          // a PLL's probe point in the first shard's run (shard_begin), or -1
 };
 
 struct Dag {
     std::vector<DagNode> nodes;
-    std::vector<int> outputs;
+    std::vector<PortRef> outputs;  // never the DAG input
     DeviceBuffer d_in;
     size_t in_size = 0;
     std::string desc;
@@ -684,6 +698,7 @@ struct Dag {
     int add(Block* blk, const int* refs, unsigned nin) {
         DagNode nd;
         nd.blk.reset(blk);
+        nd.pll = blk->as_pll();
         if (wire(nd, refs, nin) != 0) { nd.blk.release(); return -1; }
         nd.out_buf.resize((size_t)blk->num_outputs);
         nd.out_cnt.assign((size_t)blk->num_outputs, 0);
@@ -699,24 +714,34 @@ struct Dag {
         const Block& b = *nd.blk;
         if ((int)nin != b.num_inputs) { set_error("dag: %s takes %d input(s), got %u", b.name.c_str(), b.num_inputs, nin); return -1; }
         for (unsigned i = 0; i < nin; ++i) {
-            const int r = refs[i];
+            PortRef r;
             size_t esz;
-            if (r == -1) {
+            if (refs[i] == -1) {
                 if (in_size && in_size != b.in_size) { set_error("dag: the input feeds nodes of different sample sizes"); return -1; }
                 in_size = b.in_size;
                 esz = in_size;
             } else {
-                const int pn = r >> 2, pp = r & 3;
-                if (r < 0 || pn >= (int)nodes.size() || pp >= nodes[(size_t)pn].blk->num_outputs) { set_error("dag: bad input reference %d", r); return -1; }
-                esz = nodes[(size_t)pn].blk->out_size_of(pp);
+                if (decode(refs[i], &r) != 0) { set_error("dag: bad input reference %d", refs[i]); return -1; }
+                esz = node(r).blk->out_size_of(r.port);
             }
             if (esz != b.in_size) { set_error("dag: %zu-byte samples cannot feed %s (%zu-byte input)", esz, b.name.c_str(), b.in_size); return -1; }
-            nd.in_refs.push_back(r);
+            nd.ins.push_back(r);
         }
         return 0;
     }
 
-    size_t out_size(size_t k) const { return nodes[(size_t)(outputs[k] >> 2)].blk->out_size_of(outputs[k] & 3); }
+    // an ABI reference to an existing node's output port: 0, or -1 (no such port)
+    int decode(int ref, PortRef* r) const {
+        if (ref < 0 || (ref >> 2) >= (int)nodes.size() || (ref & 3) >= nodes[(size_t)(ref >> 2)].blk->num_outputs) return -1;
+        *r = PortRef{ref >> 2, ref & 3};
+        return 0;
+    }
+    const DagNode& node(PortRef r) const { return nodes[(size_t)r.node]; }
+    // where port r's samples of the current call are, and how many (the DAG input: dx, n)
+    const void* port_ptr(PortRef r, const void* dx) const { return r.is_input() ? dx : node(r).out_ptr[(size_t)r.port]; }
+    size_t port_cnt(PortRef r, size_t n) const { return r.is_input() ? n : node(r).out_cnt[(size_t)r.port]; }
+
+    size_t out_size(size_t k) const { return node(outputs[k]).blk->out_size_of(outputs[k].port); }
     // conservative: no node here produces more samples than its input times the interpolation factors on the way
     size_t max_output(size_t n) const {
         size_t m = n;
@@ -743,11 +768,10 @@ struct Dag {
         for (size_t i = 0; i < nodes.size(); ++i)
             if (run_node(i, dx, n, dy, s) != 0) return -1;
         for (size_t k = 0; k < outputs.size(); ++k) {
-            const DagNode& nd = nodes[(size_t)(outputs[k] >> 2)];
-            const size_t port = (size_t)(outputs[k] & 3), c = nd.out_cnt[port];
+            const void* p = port_ptr(outputs[k], nullptr);
+            const size_t c = port_cnt(outputs[k], 0);
             // an output listed twice: the producer wrote the first dy only
-            if (dy && c && nd.out_ptr[port] != dy[k])
-                LRB_CHECK(cudaMemcpyAsync(dy[k], nd.out_ptr[port], c * out_size(k), cudaMemcpyDeviceToDevice, s));
+            if (dy && c && p != dy[k]) LRB_CHECK(cudaMemcpyAsync(dy[k], p, c * out_size(k), cudaMemcpyDeviceToDevice, s));
             n_out[k] = c;
         }
         return 0;
@@ -760,20 +784,17 @@ struct Dag {
         DagNode& nd = nodes[i];
         ins.clear();
         *cnt = 0;
-        for (size_t j = 0; j < nd.in_refs.size(); ++j) {
-            const int r = nd.in_refs[j];
-            const void* p = r == -1 ? dx : nodes[(size_t)(r >> 2)].out_ptr[(size_t)(r & 3)];
-            const size_t c = r == -1 ? n : nodes[(size_t)(r >> 2)].out_cnt[(size_t)(r & 3)];
+        for (size_t j = 0; j < nd.ins.size(); ++j) {
+            const size_t c = port_cnt(nd.ins[j], n);
             if (j && c != *cnt) { set_error("dag: %s received inputs of different lengths (%zu, %zu)", nd.blk->name.c_str(), *cnt, c); return -1; }
             *cnt = c;
-            ins.push_back(p);
+            ins.push_back(port_ptr(nd.ins[j], dx));
         }
         const size_t mo = nd.blk->max_output(*cnt);
         for (int o = 0; o < nd.blk->num_outputs; ++o) {
-            const int ref = (int)i * 4 + o;
             void* ext = nullptr;
             for (size_t k = 0; dy && k < outputs.size() && !ext; ++k)
-                if (outputs[k] == ref) ext = dy[k];
+                if (outputs[k].node == (int)i && outputs[k].port == o) ext = dy[k];
             if (!ext) {
                 DeviceBuffer& buf = nd.out_buf[(size_t)o];
                 const size_t bytes = (mo ? mo : 1) * nd.blk->out_size_of(o);
@@ -788,8 +809,8 @@ struct Dag {
         return 0;
     }
 
-    // One node's launches.  A PLL with a probe point (sh.probe, the first rank of a sharded stream) also leaves its state
-    // there in its record.
+    // One node's launches.  A PLL with a probe point (the first rank of a sharded stream) also leaves its state there in
+    // its record.
     int run_node(size_t i, const void* dx, size_t n, void* const* dy, cudaStream_t s) {
         DagNode& nd = nodes[i];
         std::vector<const void*> ins;
@@ -797,8 +818,8 @@ struct Dag {
         void* outs[4];                 // a port is two bits of a reference
         if (node_io(i, dx, n, dy, ins, &cnt, outs, s) != 0) return -1;
         size_t no = 0;
-        if (!sh.probe.empty() && sh.probe[i] >= 0) {
-            if (static_cast<PllBlock*>(nd.blk.get())->run_probe(ins[0], cnt, outs, sh.probe[i], rec_dev(i) + 2, s) != 0) return -1;
+        if (nd.probe >= 0) {
+            if (nd.pll->run_probe(ins[0], cnt, outs, nd.probe, rec_dev(nd), s) != 0) return -1;
             no = cnt;
         } else if (nd.blk->run_multi(ins.data(), (int)ins.size(), cnt, outs, nd.blk->num_outputs, &no, s) != 0) {
             return -1;
@@ -826,10 +847,8 @@ struct Dag {
         }
         if (n) LRB_CHECK(cudaMemcpyAsync(d_in.get(), x, n * in_size, cudaMemcpyHostToDevice, s));
         if (run_nodes(d_in.get(), n, nullptr, n_out, s) != 0) return -1;
-        for (size_t k = 0; k < outputs.size(); ++k) {
-            const DagNode& nd = nodes[(size_t)(outputs[k] >> 2)];
-            if (n_out[k]) LRB_CHECK(cudaMemcpyAsync(y[k], nd.out_ptr[(size_t)(outputs[k] & 3)], n_out[k] * out_size(k), cudaMemcpyDeviceToHost, s));
-        }
+        for (size_t k = 0; k < outputs.size(); ++k)
+            if (n_out[k]) LRB_CHECK(cudaMemcpyAsync(y[k], port_ptr(outputs[k], nullptr), n_out[k] * out_size(k), cudaMemcpyDeviceToHost, s));
         LRB_CHECK(cudaStreamSynchronize(s));
         return 0;
     }
@@ -862,13 +881,9 @@ struct Dag {
     // a shard's start, less what everything behind the PLL needs of left context (from h on, the PLL's outputs reach the
     // shard's kept outputs), the loop is speculated from a lead-in over the halo (the chunk-parallel form's speculation,
     // pll.cu), checked against the left shard's state at h, re-run from that state on a miss, and the VCO output is
-    // started from the sum of the left shards' advances of the multiplied phase.
-    static constexpr int REC = 6;    // doubles per PLL: spec phi, spec freq, end phi, end sum dP, end freq, first
+    // started from the sum of the left shards' advances of the multiplied phase.  A shard's record is one
+    // PllShardRecord per PLL, in node order.
     struct ShardState {
-        std::vector<long long> probe;          // per node: the first shard's PLL probe point, or -1
-        std::vector<double> need_out;          // per node: outputs of left context its consumers and ports need
-        std::vector<char> below_pll;           // per node: a transitive consumer of a PLL
-        std::vector<int> pll_of;               // per node: index of its PLL record, or -1
         std::vector<int> plls;                 // node ids of the PLLs
         unsigned long long period = 1;         // lcm of every output port's total decimation
         double need = 0.0;                     // input samples of left context, unrounded
@@ -878,70 +893,45 @@ struct Dag {
         uint64_t start = 0;
         size_t halo = 0, n = 0;
         std::vector<size_t> skip;              // per port: outputs of the halo
-        std::vector<double> rec;               // host copy of this shard's record
         bool planned = false;
     };
     ShardState sh;
     DeviceBuffer d_rec;
-    std::vector<double> h_rec;
+    std::vector<PllShardRecord> h_rec;     // host copy of this shard's record
 
-    double* rec_dev(size_t node) { return d_rec.as<double>() + (size_t)REC * (size_t)sh.pll_of[node]; }
-    size_t record_bytes() { return plan() != 0 ? 0 : sizeof(double) * REC * sh.plls.size(); }
+    PllShardRecord* rec_dev(const DagNode& nd) { return d_rec.as<PllShardRecord>() + nd.rec; }
+    size_t record_bytes() { return plan() != 0 ? 0 : sizeof(PllShardRecord) * sh.plls.size(); }
 
     // needs, PLLs and the period, from the shape alone; -1 with the error set when the stream cannot be cut
     int plan() {
         if (sh.planned) return 0;
         if (nodes.empty() || outputs.empty()) { set_error("dag: no nodes / no outputs"); return -1; }
-        const size_t N = nodes.size();
-        sh.need_out.assign(N, 0.0);
-        sh.below_pll.assign(N, 0);
-        sh.pll_of.assign(N, -1);
         sh.plls.clear();
-        std::vector<unsigned long long> up(N, 1), down(N, 1);        // total rate at each node's output
-        for (size_t i = 0; i < N; ++i) {
-            const DagNode& nd = nodes[i];
-            const bool pll = dynamic_cast<PllBlock*>(nd.blk.get()) != nullptr;
-            unsigned long long u = 1, d = 1;
-            for (int r : nd.in_refs)
-                if (r != -1) {
-                    const size_t p = (size_t)(r >> 2);
-                    if (sh.below_pll[p] || sh.pll_of[p] >= 0) sh.below_pll[i] = 1;
-                    u = up[p]; d = down[p];
+        std::vector<Rate> rate(nodes.size());                  // total rate at each node's output
+        for (size_t i = 0; i < nodes.size(); ++i) {
+            DagNode& nd = nodes[i];
+            nd.need_out = 0.0;
+            nd.below_pll = false;
+            nd.rec = -1;
+            Rate r;
+            for (PortRef p : nd.ins)
+                if (!p.is_input()) {
+                    if (node(p).below_pll || node(p).pll) nd.below_pll = true;
+                    r = rate[(size_t)p.node];
                 }
-            if (pll && sh.below_pll[i]) { set_error("dag: %s behind another pll, the stream cannot be cut", nd.blk->name.c_str()); return -1; }
-            if (pll) { sh.pll_of[i] = (int)sh.plls.size(); sh.plls.push_back((int)i); }
-            unsigned bu, bd;
-            nd.blk->rate(&bu, &bd);
-            u *= bu; d *= bd;
-            unsigned long long a = u, c = d;
-            while (c) { const unsigned long long t = a % c; a = c; c = t; }
-            up[i] = u / a; down[i] = d / a;
+            if (nd.pll && nd.below_pll) { set_error("dag: %s behind another pll, the stream cannot be cut", nd.blk->name.c_str()); return -1; }
+            if (nd.pll) { nd.rec = (int)sh.plls.size(); sh.plls.push_back((int)i); }
+            rate[i] = r.then(*nd.blk);
         }
         sh.period = 1;
-        for (int r : outputs) {
-            const unsigned long long d = down[(size_t)(r >> 2)];
-            unsigned long long a = sh.period, c = d;
-            while (c) { const unsigned long long t = a % c; a = c; c = t; }
-            sh.period = sh.period / a * d;
-        }
-        // walk back from the ports: at a node's input, ceil(need at its output * down / up) + memory + 1
+        for (PortRef p : outputs) sh.period = std::lcm(sh.period, rate[(size_t)p.node].down);
+        // walk back from the ports: each node's need at its input from its need at its output
         sh.need = 0.0;
-        for (size_t i = N; i-- > 0;) {
-            Block* b = nodes[i].blk.get();
+        for (size_t i = nodes.size(); i-- > 0;) {
             double need;
-            if (Graph* g = dynamic_cast<Graph*>(b)) {
-                if (g->need_in(sh.need_out[i], &need) != 0) return -1;
-            } else if (PllBlock* p = dynamic_cast<PllBlock*>(b)) {
-                need = sh.need_out[i] + (double)p->warm + 1.0;     // the lead-in, behind the handoff point
-            } else {
-                const long long mem = b->memory_in();
-                if (mem < 0) { set_error("dag: %s has unbounded memory, the stream cannot be cut", b->name.c_str()); return -1; }
-                unsigned bu, bd;
-                b->rate(&bu, &bd);
-                need = std::ceil(sh.need_out[i] * (double)bd / (double)bu) + (double)mem + 1.0;
-            }
-            for (int r : nodes[i].in_refs) {
-                double& t = r == -1 ? sh.need : sh.need_out[(size_t)(r >> 2)];
+            if (nodes[i].blk->need_in(nodes[i].need_out, &need) != 0) return -1;
+            for (PortRef p : nodes[i].ins) {
+                double& t = p.is_input() ? sh.need : nodes[(size_t)p.node].need_out;
                 t = need > t ? need : t;
             }
         }
@@ -949,21 +939,14 @@ struct Dag {
         return 0;
     }
 
-    long long halo() {
-        if (plan() != 0) return -1;
-        // whole output periods of every port, and a multiple of 4 samples so that a chunk placed `halo` samples into a
-        // 16-byte aligned buffer stays 16-byte aligned (as Graph::halo)
-        const long long q = 4 * (long long)sh.period;
-        const long long h = (long long)std::ceil(sh.need);
-        return ((h + q - 1) / q) * q;
-    }
+    long long halo() { return plan() != 0 ? -1 : round_halo(sh.need, sh.period); }
 
     // every node's input index once the DAG input's first `g` samples are consumed
     std::vector<uint64_t> in_index(uint64_t g) const {
         std::vector<uint64_t> idx(nodes.size());
         for (size_t i = 0; i < nodes.size(); ++i) {
-            const int r = nodes[i].in_refs.empty() ? -1 : nodes[i].in_refs[0];
-            idx[i] = r == -1 ? g : nodes[(size_t)(r >> 2)].blk->outputs_before(idx[(size_t)(r >> 2)]);
+            const PortRef r = nodes[i].ins.empty() ? PortRef{} : nodes[i].ins[0];
+            idx[i] = r.is_input() ? g : node(r).blk->outputs_before(idx[(size_t)r.node]);
         }
         return idx;
     }
@@ -983,39 +966,37 @@ struct Dag {
 
     // the kept outputs of port k (from its node's edge buffer) to dy[k]
     int copy_port(size_t k, void* const* dy, size_t* n_out, cudaStream_t s) {
-        const DagNode& nd = nodes[(size_t)(outputs[k] >> 2)];
-        const size_t port = (size_t)(outputs[k] & 3), c = nd.out_cnt[port], sk = sh.skip[k];
+        const size_t c = port_cnt(outputs[k], 0), sk = sh.skip[k];
         if (c < sk) { set_error("dag: output %zu: the halo produced %zu outputs, expected %zu", k, c, sk); return -1; }
-        if (c > sk) LRB_CHECK(cudaMemcpyAsync(dy[k], (const char*)nd.out_ptr[port] + sk * out_size(k), (c - sk) * out_size(k),
-                                              cudaMemcpyDeviceToDevice, s));
+        if (c > sk) LRB_CHECK(cudaMemcpyAsync(dy[k], (const char*)port_ptr(outputs[k], nullptr) + sk * out_size(k),
+                                              (c - sk) * out_size(k), cudaMemcpyDeviceToDevice, s));
         n_out[k] = c - sk;
         return 0;
     }
 
     bool port_in_phase_b(size_t k) const {
-        const size_t i = (size_t)(outputs[k] >> 2);
-        return sh.below_pll[i] || sh.pll_of[i] >= 0;
+        const DagNode& nd = node(outputs[k]);
+        return nd.below_pll || nd.pll;
     }
 
     int shard_begin(const void* dx, size_t halo_n, size_t n, uint64_t start, void* const* dy, size_t* n_out, void* record,
                     size_t record_bytes_) {
         if (sc.samples) { set_error("dag: sharding runs the stream directly; switch super-chunk mode off first (set_superchunk 0)"); return -1; }
         if (plan() != 0 || check_record(record_bytes_) != 0) return -1;
-        if (halo_n % sh.period || start % sh.period) { set_error("dag: halo and start must be multiples of %llu input samples", sh.period); return -1; }
-        const bool first = halo_n == 0 || start == 0;
-        if (!first && start < halo_n) { set_error("dag: chunk starts inside the halo"); return -1; }
+        bool first;
+        if (shard_args("dag", halo_n, start, sh.period, &first) != 0) return -1;
         sh.pending = false;
         if (reset() != 0) return -1;
         cudaStream_t s = ctx().stream;
         const size_t npll = sh.plls.size();
-        if (npll && d_rec.reserve(sizeof(double) * REC * npll) != 0) return -1;
+        if (npll && d_rec.reserve(sizeof(PllShardRecord) * npll) != 0) return -1;
         const uint64_t g0 = first ? start : start - halo_n;
         if (seek(g0) != 0) return -1;
         const std::vector<uint64_t> a0 = in_index(g0), a1 = in_index(start), a2 = in_index(start + n);
         // handoff points of each PLL, as indices into this call's PLL input
         std::vector<long long> lh(nodes.size(), -1), le(nodes.size(), -1);
         for (int p : sh.plls) {
-            const long long D = (long long)std::ceil(sh.need_out[(size_t)p]);
+            const long long D = (long long)std::ceil(nodes[(size_t)p].need_out);
             lh[(size_t)p] = (long long)a1[(size_t)p] - D - (long long)a0[(size_t)p];
             le[(size_t)p] = (long long)a2[(size_t)p] - D - (long long)a0[(size_t)p];
             if (le[(size_t)p] < (first ? 0 : lh[(size_t)p])) { set_error("dag: the chunk is shorter than what follows %s needs", nodes[(size_t)p].blk->name.c_str()); return -1; }
@@ -1024,24 +1005,25 @@ struct Dag {
         int rc = 0;
         if (first) {
             // the plain run, with each PLL's state at the next shard's handoff point
-            sh.probe = le;
+            for (int p : sh.plls) nodes[(size_t)p].probe = le[(size_t)p];
             rc = run_nodes((const char*)dx + halo_n * in_size, n, dy, n_out, s);
-            sh.probe.clear();
+            for (int p : sh.plls) nodes[(size_t)p].probe = -1;
         } else {
             for (size_t k = 0; k < outputs.size(); ++k) {
-                const size_t i = (size_t)(outputs[k] >> 2);
+                const size_t i = (size_t)outputs[k].node;
                 sh.skip[k] = (size_t)(nodes[i].blk->outputs_before(a1[i]) - nodes[i].blk->outputs_before(a0[i]));
             }
             const size_t N = halo_n + n;
             for (size_t i = 0; i < nodes.size() && rc == 0; ++i) {
-                if (sh.below_pll[i]) continue;
-                if (sh.pll_of[i] < 0) { rc = run_node(i, dx, N, nullptr, s); continue; }
+                DagNode& nd = nodes[i];
+                if (nd.below_pll) continue;
+                if (!nd.pll) { rc = run_node(i, dx, N, nullptr, s); continue; }
                 std::vector<const void*> ins;
                 size_t cnt = 0;
                 void* outs[4];
                 rc = node_io(i, dx, N, nullptr, ins, &cnt, outs, s);
-                if (rc == 0) rc = static_cast<PllBlock*>(nodes[i].blk.get())->shard_loop(ins[0], cnt, (float*)outs[1], lh[i], le[i], rec_dev(i), s);
-                nodes[i].out_cnt[0] = nodes[i].out_cnt[1] = cnt;
+                if (rc == 0) rc = nd.pll->shard_loop(ins[0], cnt, (float*)outs[1], lh[i], le[i], rec_dev(nd), s);
+                nd.out_cnt[0] = nd.out_cnt[1] = cnt;
             }
             for (size_t k = 0; k < outputs.size() && rc == 0; ++k) {
                 n_out[k] = 0;
@@ -1049,15 +1031,15 @@ struct Dag {
             }
         }
         if (rc != 0) return -1;
-        h_rec.assign(REC * npll, 0.0);
+        h_rec.assign(npll, PllShardRecord{});
         if (npll) {
-            LRB_CHECK(cudaMemcpyAsync(h_rec.data(), d_rec.get(), sizeof(double) * REC * npll, cudaMemcpyDeviceToHost, s));
+            LRB_CHECK(cudaMemcpyAsync(h_rec.data(), d_rec.get(), sizeof(PllShardRecord) * npll, cudaMemcpyDeviceToHost, s));
             LRB_CHECK(cudaStreamSynchronize(s));
-            for (size_t j = 0; j < npll; ++j) {
-                h_rec[REC * j + 5] = first ? 1.0 : 0.0;
-                if (first) h_rec[REC * j] = h_rec[REC * j + 1] = 0.0;     // no speculated start
+            for (PllShardRecord& r : h_rec) {
+                r.first = first ? 1.0 : 0.0;
+                if (first) r.spec_phi = r.spec_freq = 0.0;      // no speculated start
             }
-            memcpy(record, h_rec.data(), sizeof(double) * REC * npll);
+            memcpy(record, h_rec.data(), sizeof(PllShardRecord) * npll);
         }
         sh.pending = true;
         sh.first = first;
@@ -1066,28 +1048,23 @@ struct Dag {
     }
 
     // does this shard's speculated start agree with the left shard's end state, for every PLL?
-    int shard_accepts(const double* left, const double* own) {
+    int shard_accepts(const PllShardRecord* left, const PllShardRecord* own) {
         for (size_t j = 0; j < sh.plls.size(); ++j) {
-            const double* l = left + REC * j;
-            const double* o = own + REC * j;
-            if (o[5] != 0.0) continue;                               // a first shard starts from the reset state
-            const PllBlock* p = static_cast<const PllBlock*>(nodes[(size_t)sh.plls[j]].blk.get());
-            if (!p->accepts(l[2], l[4], o[0], o[1])) return 0;
+            if (own[j].first != 0.0) continue;                      // a first shard starts from the reset state
+            const PllBlock* p = nodes[(size_t)sh.plls[j]].pll;
+            if (!p->accepts(left[j].end_phi, left[j].end_freq, own[j].spec_phi, own[j].spec_freq)) return 0;
         }
         return 1;
     }
 
-    int shard_end(const double* left, unsigned num_left, void* const* dy, size_t* n_out, void* record_out, size_t record_bytes_) {
+    int shard_end(const PllShardRecord* left, unsigned num_left, void* const* dy, size_t* n_out, void* record_out, size_t record_bytes_) {
         if (!sh.pending) { set_error("dag: shard_end without shard_begin"); return -1; }
         if (check_record(record_bytes_) != 0) return -1;
         const size_t npll = sh.plls.size();
         cudaStream_t s = ctx().stream;
         if (sh.first) {
-            for (size_t k = 0; k < outputs.size(); ++k) {
-                const DagNode& nd = nodes[(size_t)(outputs[k] >> 2)];
-                n_out[k] = nd.out_cnt[(size_t)(outputs[k] & 3)];
-            }
-            if (npll) memcpy(record_out, h_rec.data(), sizeof(double) * REC * npll);
+            for (size_t k = 0; k < outputs.size(); ++k) n_out[k] = port_cnt(outputs[k], 0);
+            if (npll) memcpy(record_out, h_rec.data(), sizeof(PllShardRecord) * npll);
             sh.pending = false;
             return 0;
         }
@@ -1095,42 +1072,36 @@ struct Dag {
         bool rerun = false;
         int rc = 0;
         for (size_t j = 0; j < npll && rc == 0; ++j) {
-            const size_t i = (size_t)sh.plls[j];
-            PllBlock* p = static_cast<PllBlock*>(nodes[i].blk.get());
-            const double* l = left + REC * npll * (size_t)(num_left - 1) + REC * j;
-            const double* o = h_rec.data() + REC * j;
-            // the multiplied phase at the handoff point: the left shards' advances, summed as pll_verify_kernel sums bases
-            double base = 0.0;
-            for (unsigned r = 0; r < num_left; ++r) {
-                base = base + left[(size_t)REC * (npll * r + j) + 3];
-                base = base > 6.283185307179586476925286766559 ? base - 6.283185307179586476925286766559 : base;
-                base = base < -6.283185307179586476925286766559 ? base + 6.283185307179586476925286766559 : base;
-            }
-            const int r = nodes[i].in_refs[0];
-            const void* x = r == -1 ? sh.dx : nodes[(size_t)(r >> 2)].out_ptr[(size_t)(r & 3)];
-            if (!p->accepts(l[2], l[4], o[0], o[1])) {
+            DagNode& nd = nodes[(size_t)sh.plls[j]];
+            const PllShardRecord& l = left[npll * (size_t)(num_left - 1) + j];
+            const PllShardRecord& o = h_rec[j];
+            const double base = PllBlock::fold_advances(left, num_left, npll, j);
+            if (!nd.pll->accepts(l.end_phi, l.end_freq, o.spec_phi, o.spec_freq)) {
                 rerun = true;
-                rc = p->shard_rerun(x, (float*)nodes[i].out_ptr[1], l[2], l[4], rec_dev(i), s);
+                rc = nd.pll->shard_rerun(port_ptr(nd.ins[0], sh.dx), (float*)nd.out_ptr[1], l.end_phi, l.end_freq, rec_dev(nd), s);
             }
-            if (rc == 0) rc = p->shard_out((const float*)nodes[i].out_ptr[1], (float2*)nodes[i].out_ptr[0], base, s);
+            if (rc == 0) rc = nd.pll->shard_out((const float*)nd.out_ptr[1], (float2*)nd.out_ptr[0], base, s);
         }
         const size_t N = sh.halo + sh.n;
         for (size_t i = 0; i < nodes.size() && rc == 0; ++i)
-            if (sh.below_pll[i]) rc = run_node(i, sh.dx, N, nullptr, s);
+            if (nodes[i].below_pll) rc = run_node(i, sh.dx, N, nullptr, s);
         for (size_t k = 0; k < outputs.size() && rc == 0; ++k) {
             if (port_in_phase_b(k)) rc = copy_port(k, dy, n_out, s);
-            else n_out[k] = nodes[(size_t)(outputs[k] >> 2)].out_cnt[(size_t)(outputs[k] & 3)] - sh.skip[k];
+            else n_out[k] = port_cnt(outputs[k], 0) - sh.skip[k];
         }
         if (rc != 0) return -1;
         if (rerun) {
-            // only the end states and sums are the device's: the speculated start and the first-shard flag stay the host's
-            std::vector<double> dev(REC * npll);
-            LRB_CHECK(cudaMemcpyAsync(dev.data(), d_rec.get(), sizeof(double) * REC * npll, cudaMemcpyDeviceToHost, s));
+            // only the end states are the device's: the speculated start and the first-shard flag stay the host's
+            std::vector<PllShardRecord> dev(npll);
+            LRB_CHECK(cudaMemcpyAsync(dev.data(), d_rec.get(), sizeof(PllShardRecord) * npll, cudaMemcpyDeviceToHost, s));
             LRB_CHECK(cudaStreamSynchronize(s));
-            for (size_t j = 0; j < npll; ++j)
-                for (int f = 2; f < 5; ++f) h_rec[REC * j + f] = dev[REC * j + f];
+            for (size_t j = 0; j < npll; ++j) {
+                h_rec[j].end_phi = dev[j].end_phi;
+                h_rec[j].end_dP = dev[j].end_dP;
+                h_rec[j].end_freq = dev[j].end_freq;
+            }
         }
-        if (npll) memcpy(record_out, h_rec.data(), sizeof(double) * REC * npll);
+        if (npll) memcpy(record_out, h_rec.data(), sizeof(PllShardRecord) * npll);
         sh.pending = false;
         return rerun ? 1 : 0;
     }
@@ -1314,11 +1285,10 @@ int lrb200_dag_add_graph(lrb200_dag_t* d, lrb200_graph_t* g, int input) {
 int lrb200_dag_set_outputs(lrb200_dag_t* d, const int* outputs, unsigned num_outputs) {
     if (!d || !outputs || !num_outputs) { set_error("dag_set_outputs: null argument"); return -1; }
     if (d->d.sc.samples) { set_error("dag_set_outputs: the super-chunk slots are sized for the outputs; set them first"); return -1; }
-    for (unsigned k = 0; k < num_outputs; ++k) {
-        const int r = outputs[k];
-        if (r < 0 || (r >> 2) >= (int)d->d.nodes.size() || (r & 3) >= d->d.nodes[(size_t)(r >> 2)].blk->num_outputs) { set_error("dag_set_outputs: bad reference %d", r); return -1; }
-    }
-    d->d.outputs.assign(outputs, outputs + num_outputs);
+    std::vector<PortRef> refs(num_outputs);
+    for (unsigned k = 0; k < num_outputs; ++k)
+        if (d->d.decode(outputs[k], &refs[k]) != 0) { set_error("dag_set_outputs: bad reference %d", outputs[k]); return -1; }
+    d->d.outputs = std::move(refs);
     d->d.sh.planned = false;
     return 0;
 }
@@ -1377,13 +1347,13 @@ int lrb200_dag_shard_begin(lrb200_dag_t* d, const void* dx, size_t halo, size_t 
 int lrb200_dag_shard_accepts(lrb200_dag_t* d, const void* left_record, const void* record, size_t record_bytes) {
     if (!d || (record_bytes && (!left_record || !record))) { set_error("dag_shard_accepts: null argument"); return -1; }
     if (d->d.check_record(record_bytes) != 0) return -1;
-    return d->d.shard_accepts((const double*)left_record, (const double*)record);
+    return d->d.shard_accepts((const PllShardRecord*)left_record, (const PllShardRecord*)record);
 }
 
 int lrb200_dag_shard_end(lrb200_dag_t* d, const void* left_records, unsigned num_left, void* const* dy, size_t* n_out,
                          void* record_out, size_t record_bytes) {
     if (!d || !dy || !n_out || (record_bytes && (!record_out || (num_left && !left_records)))) { set_error("dag_shard_end: null argument"); return -1; }
-    return d->d.shard_end((const double*)left_records, num_left, dy, n_out, record_out, record_bytes);
+    return d->d.shard_end((const PllShardRecord*)left_records, num_left, dy, n_out, record_out, record_bytes);
 }
 
 const char* lrb200_dag_describe(const lrb200_dag_t* d) { return d ? d->d.desc.c_str() : ""; }

@@ -10,6 +10,7 @@
 #include "blocks.h"
 
 #include <cmath>
+#include <cstddef>
 
 namespace lrb {
 
@@ -232,10 +233,14 @@ void pll_thresholds(double alpha, double beta, double mult, double* dphi, double
 // ---- time-chunk sharding of a device DAG (graph.cu, Dag::shard_begin / shard_end).  A shard's PLL input holds, before
 // the handoff point lh, a lead-in the left rank's samples fill; the loop is speculated from lh as pll_sim_kernel
 // speculates a chunk, and its state at lh, at the next rank's handoff point and the wrapped sum of the multiplied
-// phase's advances between them go to the shard's record: {spec phi, spec freq, end phi, end sum dP, end freq, first}.
+// phase's advances between them go to the shard's PllShardRecord.
+
+// d_shard's (phi, sum of dP, freq) lands on a record's end state in one 24-byte copy
+static_assert(offsetof(PllShardRecord, end_freq) - offsetof(PllShardRecord, end_phi) == 2 * sizeof(double), "end state");
 
 // the lead-in of pll_sim_kernel over x[lh - W, lh): st = (phi, 0, freq) and the record's speculated start
-__global__ void pll_lead_kernel(const float2* __restrict__ x, long long lh, long long W, PllParams P, double* st, double* rec) {
+__global__ void pll_lead_kernel(const float2* __restrict__ x, long long lh, long long W, PllParams P, double* st,
+                                PllShardRecord* rec) {
     if (blockIdx.x != 0 || threadIdx.x != 0) return;
     const float2 x0 = x[lh - W];
     double phi = (double)atan2f(x0.y, x0.x), freq = 0.5 * (P.fmin + P.fmax);
@@ -244,7 +249,7 @@ __global__ void pll_lead_kernel(const float2* __restrict__ x, long long lh, long
         pll_clamp(freq, P);
     }
     st[0] = phi; st[1] = 0.0; st[2] = freq;
-    rec[0] = phi; rec[1] = freq;
+    rec->spec_phi = phi; rec->spec_freq = freq;
 }
 
 // one chunk of n samples in the sequential form from st, with its summary: what pll_verify_kernel makes of a re-run
@@ -381,14 +386,24 @@ bool PllBlock::accepts(double tphi, double tfreq, double phi0, double freq0) con
     return std::fabs(d) <= dphi && std::fabs(tfreq - freq0) <= dfreq;
 }
 
-int PllBlock::run_probe(const void* x, size_t n, void* const* dy, long long split, double* state_out, cudaStream_t s) {
+double PllBlock::fold_advances(const PllShardRecord* lefts, unsigned num_left, size_t stride, size_t j) {
+    double base = 0.0;
+    for (unsigned r = 0; r < num_left; ++r) {
+        base = base + lefts[stride * r + j].end_dP;
+        base = base > PLL_TWO_PI ? base - PLL_TWO_PI : base;
+        base = base < -PLL_TWO_PI ? base + PLL_TWO_PI : base;
+    }
+    return base;
+}
+
+int PllBlock::run_probe(const void* x, size_t n, void* const* dy, long long split, PllShardRecord* rec, cudaStream_t s) {
     if (split < 0 || split > (long long)n) { set_error("pll: probe at %lld outside a call of %zu samples", split, n); return -1; }
     size_t no = 0;
     if (parallel(n)) {
         if (run_multi(&x, 1, n, dy, 2, &no, s) != 0) return -1;
         const long long L = chunk_len();
         pll_probe_kernel<<<1, 32, 0, s>>>((const float2*)x, L, d_chunks.as<PllChunk>(), (int)(((long long)n + L - 1) / L), split, P,
-                                          state_out);
+                                          &rec->end_phi);
         count_launch();
         LRB_CHECK(cudaGetLastError());
         return 0;
@@ -399,7 +414,7 @@ int PllBlock::run_probe(const void* x, size_t n, void* const* dy, long long spli
         pll_kernel<<<1, 32, 0, s>>>((const float2*)x, split, (float2*)dy[0], (float*)dy[1], st, P);
         count_launch();
     }
-    LRB_CHECK(cudaMemcpyAsync(state_out, st, 3 * sizeof(double), cudaMemcpyDeviceToDevice, s));
+    LRB_CHECK(cudaMemcpyAsync(&rec->end_phi, st, 3 * sizeof(double), cudaMemcpyDeviceToDevice, s));
     if ((long long)n > split) {
         pll_kernel<<<1, 32, 0, s>>>((const float2*)x + split, (long long)n - split, (float2*)dy[0] + split, (float*)dy[1] + split, st, P);
         count_launch();
@@ -433,7 +448,7 @@ int PllBlock::shard_range(const ShardRange& r, const void* x, float* err, bool r
     return 0;
 }
 
-int PllBlock::shard_loop(const void* x, size_t n, float* err, long long lh, long long le, double* rec, cudaStream_t s) {
+int PllBlock::shard_loop(const void* x, size_t n, float* err, long long lh, long long le, PllShardRecord* rec, cudaStream_t s) {
     if (lh < warm || le < lh || le > (long long)n) {
         set_error("pll: handoff points %lld, %lld of a %zu-sample shard leave no %lld-sample lead-in", lh, le, n, warm);
         return -1;
@@ -455,17 +470,17 @@ int PllBlock::shard_loop(const void* x, size_t n, float* err, long long lh, long
     pll_lead_kernel<<<1, 32, 0, s>>>((const float2*)x, lh, warm, P, d_shard.as<double>(), rec);
     count_launch();
     if (shard_range(rng[0], x, err, false, s) != 0) return -1;
-    LRB_CHECK(cudaMemcpyAsync(rec + 2, d_shard.get(), 3 * sizeof(double), cudaMemcpyDeviceToDevice, s));
+    LRB_CHECK(cudaMemcpyAsync(&rec->end_phi, d_shard.get(), 3 * sizeof(double), cudaMemcpyDeviceToDevice, s));
     if (shard_range(rng[1], x, err, false, s) != 0) return -1;
     consumed += n;
     return 0;
 }
 
-int PllBlock::shard_rerun(const void* x, float* err, double tphi, double tfreq, double* rec, cudaStream_t s) {
+int PllBlock::shard_rerun(const void* x, float* err, double tphi, double tfreq, PllShardRecord* rec, cudaStream_t s) {
     const double h[3] = {tphi, 0.0, tfreq};
     LRB_CHECK(cudaMemcpyAsync(d_shard.get(), h, sizeof(h), cudaMemcpyHostToDevice, s));
     if (shard_range(rng[0], x, err, true, s) != 0) return -1;
-    LRB_CHECK(cudaMemcpyAsync(rec + 2, d_shard.get(), 3 * sizeof(double), cudaMemcpyDeviceToDevice, s));
+    LRB_CHECK(cudaMemcpyAsync(&rec->end_phi, d_shard.get(), 3 * sizeof(double), cudaMemcpyDeviceToDevice, s));
     return shard_range(rng[1], x, err, true, s);
 }
 
