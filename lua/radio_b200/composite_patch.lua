@@ -5,8 +5,9 @@
 -- MAXIMAL LINEAR RUN of GPU blocks in the crawled connection graph is collapsed into ONE lrb200 flow graph:
 -- one process() call per source vector, device-resident intermediates, fused kernels, H2D/D2H only at the
 -- two ends of the run.  Before that, every connected NON-linear set of GPU blocks with a single outside feed (the WBFM
--- stereo demodulator: two-input blocks, the PLL's two outputs, fan-outs) becomes ONE device DAG (GPUDagBlock, lrb200_dag_*),
--- with the raw file source that feeds it alone absorbed as its first node.
+-- stereo demodulator: two-input blocks, the PLL's two outputs, fan-outs), and every group of sets that share one outside
+-- feed (several receivers on one source), becomes ONE device DAG (GPUDagBlock, lrb200_dag_*), with the raw file source
+-- that feeds it alone absorbed as its first node.
 -- CPU blocks, and multi-input blocks or fan-out points outside such a set, stay ordinary blocks at the edges.
 --
 --   local top = radio.CompositeBlock(); top:connect(...); top:run()   -- unchanged user code
@@ -167,7 +168,7 @@ function M.collapse_gpu_runs(connections, substitutes)
 end
 
 --- A connected, NON-linear set of GPU blocks (a two-input block, PLLBlock's two outputs or a fan-out inside the set) fed by
--- ONE outside output port, as one device DAG (lrb200_dag_*): every edge between the members is a device buffer, the only
+-- ONE outside output port, or the sets that share one such port, as one device DAG (lrb200_dag_*): every edge between the members is a device buffer, the only
 -- host traffic is the set's input and its outputs.  Linear runs inside the set become fused flow graphs
 -- (lrb200_dag_add_graph), everything else single nodes (lrb200_dag_add_block).  A node's output k is referenced as
 -- node * 4 + k, the DAG's own input as -1 (include/lrb200.h).  An absorbed raw file source (IQFileSource, RealFileSource
@@ -304,8 +305,9 @@ end
 
 M.GPUDagBlock = GPUDagBlock
 
---- Planning step: the connected sets of GPU blocks that are not a straight line and have exactly one outside feed.
--- Returns an array of {members = {blocks in evaluation order}, ext_in = OutputPort, ext_out = {OutputPort, ...}}.
+--- Planning step: the connected sets of GPU blocks with exactly one outside feed that are not a straight line, and the
+-- sets (straight lines and single blocks included) that share one outside feed, merged into one: several receivers on
+-- one source become one DAG, so the source's samples cross PCIe once.  Returns an array of {members = {blocks in evaluation order}, ext_in = OutputPort, ext_out = {OutputPort, ...}}.
 function M.plan_gpu_dags(connections)
     local gpu, order = {}, {}                             -- set of GPU blocks; all of them in a stable order
     local function note(b)
@@ -327,7 +329,7 @@ function M.plan_gpu_dags(connections)
             adj[c][a] = true
         end
     end
-    local seen, plans = {}, {}
+    local seen, feeds_in_order, by_feed = {}, {}, {}      -- the sets with one outside feed, grouped by that feed
     for _, b in ipairs(order) do
         if not seen[b] then
             -- connected component
@@ -355,40 +357,59 @@ function M.plan_gpu_dags(connections)
             for c, _ in pairs(comp) do
                 if #c.inputs > 1 or #c.outputs > 1 then nonlinear = true end
             end
-            -- outside feeds and outside readers
+            -- outside feeds
             local feeds, nfeeds, ext_in = {}, 0, nil
-            local read_outside = {}
             for input, output in pairs(connections) do
                 if comp[input.owner] and not comp[output.owner] and not feeds[output] then
                     feeds[output] = true
                     nfeeds = nfeeds + 1
                     ext_in = output
                 end
+            end
+            if nfeeds == 1 then
+                if not by_feed[ext_in] then
+                    by_feed[ext_in] = {}
+                    feeds_in_order[#feeds_in_order + 1] = ext_in
+                end
+                table.insert(by_feed[ext_in], {comp = comp, nonlinear = count >= 2 and nonlinear})
+            end
+        end
+    end
+    -- one candidate per feed: a non-linear set, or the sets (receivers) that share it; a lone straight line is left to
+    -- collapse_gpu_runs and several outside feeds to the host scheduler
+    local plans = {}
+    for _, ext_in in ipairs(feeds_in_order) do
+        local sets = by_feed[ext_in]
+        if #sets >= 2 or sets[1].nonlinear then
+            local comp = {}
+            for _, s in ipairs(sets) do
+                for c, _ in pairs(s.comp) do comp[c] = true end
+            end
+            -- members in evaluation order: depth-first over the producers inside the set
+            local members, placed = {}, {}
+            local function place(c)
+                if placed[c] then return end
+                placed[c] = true
+                for _, p in ipairs(c.inputs) do
+                    local up = connections[p].owner
+                    if comp[up] then place(up) end
+                end
+                members[#members + 1] = c
+            end
+            for _, c in ipairs(order) do
+                if comp[c] then place(c) end
+            end
+            local read_outside = {}
+            for input, output in pairs(connections) do
                 if comp[output.owner] and not comp[input.owner] then read_outside[output] = true end
             end
-            if count >= 2 and nonlinear and nfeeds == 1 then
-                -- members in evaluation order: depth-first over the producers inside the set
-                local members, placed = {}, {}
-                local function place(c)
-                    if placed[c] then return end
-                    placed[c] = true
-                    for _, p in ipairs(c.inputs) do
-                        local up = connections[p].owner
-                        if comp[up] then place(up) end
-                    end
-                    members[#members + 1] = c
+            local ext_out = {}
+            for _, c in ipairs(members) do
+                for _, p in ipairs(c.outputs) do
+                    if read_outside[p] then ext_out[#ext_out + 1] = p end
                 end
-                for _, c in ipairs(order) do
-                    if comp[c] then place(c) end
-                end
-                local ext_out = {}
-                for _, c in ipairs(members) do
-                    for _, p in ipairs(c.outputs) do
-                        if read_outside[p] then ext_out[#ext_out + 1] = p end
-                    end
-                end
-                if #ext_out > 0 then plans[#plans + 1] = {members = members, ext_in = ext_in, ext_out = ext_out} end
             end
+            if #ext_out > 0 then plans[#plans + 1] = {members = members, ext_in = ext_in, ext_out = ext_out} end
         end
     end
     return plans

@@ -495,10 +495,12 @@ class CompositeBlock(Block):
     # GPU scheduler: maximal linear GPU runs -> GPUChainBlock, then round-robin over the reduced graph
     # ---------------------------------------------------------------------------------------------
     def _plan_gpu_dags(self):
-        """Pure planning step: connected sets of GPU blocks that are NOT a straight line (they contain a multi-port block
-        or an internal fan-out), fed by exactly one external output port -- candidates for ONE device DAG (lrb200_dag_*),
-        every edge in device memory.  Returns [(members in evaluation order, external producer port, [member output ports
-        read from outside])]."""
+        """Pure planning step: the candidates for ONE device DAG (lrb200_dag_*), every edge in device memory.  A connected
+        set of GPU blocks fed by exactly one external output port is one when it is NOT a straight line (it contains a
+        multi-port block or an internal fan-out); the sets that share one such feed -- receivers on one source, straight
+        lines and single blocks included -- are merged into one candidate, so the shared input crosses PCIe once.  Sets
+        with several external feeds stay on the host scheduler.  Returns [(members in evaluation order, external producer
+        port, [member output ports read from outside])]."""
         orig = self._all_connections
         gpu = [b for b in self._concrete_order if isinstance(b, GPUBlock) and b.inputs and b.outputs]
         gset = set(gpu)
@@ -507,7 +509,7 @@ class CompositeBlock(Block):
             if inp.owner in gset and outp.owner in gset:
                 adj[inp.owner].add(outp.owner)
                 adj[outp.owner].add(inp.owner)
-        seen, plans = set(), []
+        seen, by_feed = set(), {}                            # external feed -> [(set, non-linear)]
         for b in gpu:
             if b in seen:
                 continue
@@ -519,13 +521,18 @@ class CompositeBlock(Block):
                 comp.add(c)
                 todo.extend(adj[c] - comp)
             seen |= comp
-            members = [m for m in self._concrete_order if m in comp]
-            fan_out = any(sum(1 for i, o in orig.items() if o is p and i.owner in comp) > 1 for m in members for p in m.outputs)
-            if len(members) < 2 or not (fan_out or any(len(m.inputs) > 1 or len(m.outputs) > 1 for m in members)):
-                continue                                     # a straight line: the chain planner's business
-            ext_in = {orig[p] for m in members for p in m.inputs if orig[p].owner not in comp}
+            ext_in = {orig[p] for m in comp for p in m.inputs if orig[p].owner not in comp}
             if len(ext_in) != 1:
                 continue                                     # several external feeds: stays a host-level graph
+            fan_out = any(sum(1 for i, o in orig.items() if o is p and i.owner in comp) > 1 for m in comp for p in m.outputs)
+            nonlinear = len(comp) >= 2 and (fan_out or any(len(m.inputs) > 1 or len(m.outputs) > 1 for m in comp))
+            by_feed.setdefault(next(iter(ext_in)), []).append((comp, nonlinear))
+        plans = []
+        for ext_in, sets in by_feed.items():
+            if len(sets) == 1 and not sets[0][1]:
+                continue                                     # a lone straight line: the chain planner's business
+            comp = set().union(*(s for s, _ in sets))
+            members = [m for m in self._concrete_order if m in comp]
             ext_out = []
             for m in members:
                 for p in m.outputs:
@@ -533,7 +540,7 @@ class CompositeBlock(Block):
                         ext_out.append(p)
             if not ext_out:
                 continue
-            plans.append((members, next(iter(ext_in)), ext_out))
+            plans.append((members, ext_in, ext_out))
         return plans
 
     def _plan_gpu_runs(self, exclude=()):
@@ -577,8 +584,8 @@ class CompositeBlock(Block):
 
     def _collapse_gpu_runs(self, fuse, superchunk, device_dag=True):
         """Rewrite (self._all_connections, self._concrete_order): every planned device DAG becomes one GPUDagBlock, every
-        planned run one GPUChainBlock; a raw file source feeding only a run or a DAG, and a raw file sink fed only by a run,
-        are absorbed as its first / last stage."""
+        planned run one GPUChainBlock; a raw file source feeding only a run or a DAG (several receivers merged into one DAG
+        included), and a raw file sink fed only by a run, are absorbed as its first / last stage."""
         orig = self._all_connections          # lookups use the untouched map; the rewrite goes into `conns`
         conns = dict(orig)
         consumers = {}
@@ -846,8 +853,9 @@ class GPUChainBlock(Block):
 
 
 class GPUDagBlock(Block):
-    """A connected, non-linear set of GPU blocks as ONE device DAG (lrb200_dag_*): every edge between them is a device
-    buffer; the only host traffic is the set's single input and its outputs.  Linear runs inside the set are added as fused
+    """A connected, non-linear set of GPU blocks, or the sets that share one external feed (receivers on one source), as ONE
+    device DAG (lrb200_dag_*): every edge between them is a device buffer; the only host traffic is the single input and
+    the outputs.  Linear runs inside the set are added as fused
     lrb200 flow graphs, the rest (two-input blocks, PLL, lone blocks) as single nodes.  An absorbed raw file source makes it
     a source block: the file's own bytes cross PCIe and the source's converter is the DAG's first node.  With `superchunk`
     the host vectors are packed into super-chunks (lrb200_dag_set_superchunk) and flush() drains them at end of stream."""
