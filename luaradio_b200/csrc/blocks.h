@@ -14,6 +14,8 @@
 namespace lrb {
 
 struct PllBlock;
+struct HostBoundary;                  // graph.cu: the host <-> device boundary of a device run
+struct HostBoundaryFree { void operator()(HostBoundary* h) const; };
 
 struct Block {
     std::string name;
@@ -36,7 +38,9 @@ struct Block {
     int execute_multi(const void* const* x, int nin, size_t n, void* const* y, int nout, size_t* n_out);
     int execute(const void* x, size_t n, void* y, size_t* n_out) { return execute_multi(&x, 1, n, &y, 1, n_out); }
     virtual size_t out_size_of(int port) const { (void)port; return out_size; }    // element size of output port `port`
-    std::vector<DeviceBuffer> staging;  // host-mode staging of execute_multi: nin + nout grow-only device buffers
+    // what execute_multi stages host vectors through without LRB200_DEVICE, made by the first such call; a Graph's for
+    // lrb200_graph_execute and super-chunk mode
+    std::unique_ptr<HostBoundary, HostBoundaryFree> host;
     // Carried state: init() declares each buffer once with carry(), which allocates it zeroed.  reset() zeroes exactly
     // the declared buffers, puts every ping-pong index back to 0 and sets consumed = 0; a graph zeroes every stage's
     // buffers with ONE kernel (a 256 Mi-sample chain step is ~1 ms: a dozen cudaMemsetAsync nodes per step were 1.5 % of

@@ -57,53 +57,8 @@ static int ensure_init() {
 }
 
 // ---------------------------------------------------------------------------------------------
-// Block base: host-pointer (drop-in) mode stages through grow-only device buffers in chunks.
+// Block base: carried state (the host mode, Block::execute_multi, is in graph.cu beside HostBoundary)
 // ---------------------------------------------------------------------------------------------
-static constexpr size_t HOST_CHUNK = (size_t)1 << 24;   // samples per staged chunk in host mode
-
-int Block::execute_multi(const void* const* x, int nin, size_t n, void* const* y, int nout, size_t* n_out) {
-    cudaStream_t s = ctx().stream;
-    if (nin != num_inputs || nout != num_outputs) {
-        set_error("%s: expected %d input(s) and %d output(s), got %d and %d", name.c_str(), num_inputs, num_outputs, nin, nout);
-        return -1;
-    }
-    size_t produced = 0;
-    if (dev_ptrs) {
-        if (run_multi(x, nin, n, y, nout, &produced, s) != 0) return -1;
-        if (n_out) *n_out = produced;
-        return 0;
-    }
-    staging.resize((size_t)(nin + nout));
-    size_t done = 0;
-    std::vector<const void*> din((size_t)nin);
-    std::vector<void*> dout((size_t)nout);
-    while (done < n) {
-        const size_t nc = n - done < HOST_CHUNK ? n - done : HOST_CHUNK;
-        const size_t mo = max_output(nc);
-        for (int i = 0; i < nin; ++i) {
-            DeviceBuffer& b = staging[(size_t)i];
-            if (b.reserve(nc * in_size) != 0) return -1;
-            LRB_CHECK(cudaMemcpyAsync(b.get(), (const char*)x[i] + done * in_size, nc * in_size, cudaMemcpyHostToDevice, s));
-            din[(size_t)i] = b.get();
-        }
-        for (int o = 0; o < nout; ++o) {
-            DeviceBuffer& b = staging[(size_t)(nin + o)];
-            if (b.reserve((mo ? mo : 1) * out_size_of(o)) != 0) return -1;
-            dout[(size_t)o] = b.get();
-        }
-        size_t no = 0;
-        if (run_multi(din.data(), nin, nc, dout.data(), nout, &no, s) != 0) return -1;
-        for (int o = 0; o < nout; ++o)
-            if (no) LRB_CHECK(cudaMemcpyAsync((char*)y[o] + produced * out_size_of(o), dout[(size_t)o], no * out_size_of(o), cudaMemcpyDeviceToHost, s));
-        // the staging buffers are reused by the next chunk: drain before overwriting them
-        LRB_CHECK(cudaStreamSynchronize(s));
-        produced += no;
-        done += nc;
-    }
-    if (n_out) *n_out = produced;
-    return 0;
-}
-
 int Block::carry(DeviceBuffer& buf, size_t bytes) {
     if (buf.alloc_zeroed(bytes) != 0) return -1;
     carried.push_back({buf.get(), bytes});

@@ -167,129 +167,276 @@ static int fuse_iir_decimator(const Blocks& blocks, size_t i, Rewrite* out) {
 static const Rule FUSION_RULES[] = {fuse_tuner, fuse_rotator_overlap_save, fuse_interpolator, fuse_noble_identity,
                                    fuse_fir_decimator, fuse_iir_decimator};
 
-// Super-chunk mode (SURVEY.md 8e "streaming mode") of a linear graph or a DAG: small host vectors are packed into pinned
-// slots of `samples` input samples; a full slot is processed asynchronously while the next one fills, and its outputs (one
-// stream per output port) are handed back when that next slot is submitted (or at flush) -- the per-vector cost is one
-// host memcpy instead of copies + launches + a sync.  Every port's outputs come from the same slots.
-struct SuperChunk {
-    // device in / outs of one slot, asynchronous on s: dy[k] receives n_out[k] samples of port k
-    using Run = std::function<int(const void* dx, size_t n, void* const* dy, size_t* n_out, cudaStream_t s)>;
+// The host <-> device boundary of a device run: a linear graph, a device DAG, or a block created without LRB200_DEVICE.
+// The owner gives its run, a bound on a run's outputs per port, its ports' element sizes and its chunk length.  A host
+// call of at most one chunk is one upload per input, the run, one download per output and one synchronize, all on the
+// library stream (every call of the reference's per-vector regime, pipe.lua:73: nothing to overlap); a longer call is
+// cut into chunks pipelined over two slots on three streams, so that chunk i + 1 uploads while chunk i runs and chunk
+// i - 1 downloads.  Where a stream is cut changes output bits (PllBlock::parallel and FirBlock::path choose by call
+// length, the IIR scan places its warm-up restarts from a call's start), so each owner keeps its own chunk length.
+// Super-chunk mode (SURVEY.md 8e "streaming mode"), for an owner with one input: small host vectors are packed into
+// pinned slots of `samples` input samples; a full slot is processed asynchronously while the next one fills, and its
+// outputs (one stream per output port) are handed back when that next slot is submitted (or at flush) -- the per-vector
+// cost is one host memcpy instead of copies + launches + a sync.  Every port's outputs come from the same slots.  While
+// the mode is on, the stream runs through the slots only: a direct device or shard run is refused, and a reset waits for
+// and drops the slots in flight and the partial slot.
+struct HostBoundary {
+    // device ins / outs of one run of n samples, asynchronous on s: dy[k] receives n_out[k] samples of port k
+    using Run = std::function<int(const void* const* dx, size_t n, void* const* dy, size_t* n_out, cudaStream_t s)>;
     struct HostFree { void operator()(char* p) const { cudaFreeHost(p); } };
     using PinnedSlot = std::unique_ptr<char, HostFree>;
-    size_t samples = 0;                     // input samples per slot; 0 = off
-    size_t in_size = 0;
-    std::vector<size_t> out_size, outcap;   // per port: bytes per sample, samples a slot can produce
+    Run run;
+    std::function<size_t(size_t)> max_out;        // samples any output port may receive from a run of n inputs
+    std::vector<size_t> in_size, out_size;        // bytes per sample of each input and output port
+    size_t chunk;                                 // input samples per chunk of a host call
+    std::vector<DeviceBuffer> din[2], dout[2];    // per slot: the device staging of each port
+    std::vector<const void*> pin[2];
+    std::vector<void*> pout[2];
+    cudaStream_t s_h2d = nullptr, s_d2h = nullptr;   // the copy streams of calls longer than one chunk
+    cudaEvent_t ev_h2d[2] = {nullptr, nullptr}, ev_comp[2] = {nullptr, nullptr}, ev_d2h[2] = {nullptr, nullptr};
+    // super-chunk mode
+    size_t samples = 0;                           // input samples per slot; 0 = off
+    size_t outcap = 0;                            // samples a slot can produce in any port
     PinnedSlot hin[2];
     std::vector<PinnedSlot> hout[2];
-    DeviceBuffer din[2];
-    std::vector<DeviceBuffer> dout[2];
     cudaEvent_t done[2] = {nullptr, nullptr};
     bool pending[2] = {false, false};
     std::vector<size_t> nout[2];
     size_t fill = 0;
     int cur = 0;
+    bool fed = false;                             // an execute since the mode was set, or since the last flush / reset
 
-    ~SuperChunk() { release(); }
-    bool busy() const { return pending[0] || pending[1] || fill; }
-    size_t ports() const { return out_size.size(); }
+    HostBoundary(Run r, std::function<size_t(size_t)> mo, size_t chunk_) : run(std::move(r)), max_out(std::move(mo)), chunk(chunk_) {}
+    ~HostBoundary() {
+        release();
+        for (int i = 0; i < 2; ++i)
+            for (cudaEvent_t e : {ev_h2d[i], ev_comp[i], ev_d2h[i]})
+                if (e) cudaEventDestroy(e);
+        if (s_h2d) cudaStreamDestroy(s_h2d);
+        if (s_d2h) cudaStreamDestroy(s_d2h);
+    }
 
+    // launches in flight may still read a staging buffer that grows: the device drains first
+    static int grow(DeviceBuffer& b, size_t bytes) {
+        if (bytes <= b.capacity()) return 0;
+        LRB_CHECK(cudaDeviceSynchronize());
+        return b.reserve(bytes);
+    }
+    // the slot's device staging for a run of n inputs
+    int reserve(int slot, size_t n) {
+        const size_t mo = max_out(n);
+        din[slot].resize(in_size.size());
+        dout[slot].resize(out_size.size());
+        pin[slot].resize(in_size.size());
+        pout[slot].resize(out_size.size());
+        for (size_t i = 0; i < in_size.size(); ++i) {
+            if (grow(din[slot][i], (n ? n : 1) * in_size[i]) != 0) return -1;
+            pin[slot][i] = din[slot][i].get();
+        }
+        for (size_t k = 0; k < out_size.size(); ++k) {
+            if (grow(dout[slot][k], (mo ? mo : 1) * out_size[k]) != 0) return -1;
+            pout[slot][k] = dout[slot][k].get();
+        }
+        return 0;
+    }
+    // one run through the slot on s: the host ins x[i] up, the run, the outs down to y[k] (no synchronize)
+    int stage(int slot, const void* const* x, size_t n, void* const* y, size_t* n_out, cudaStream_t s) {
+        for (size_t i = 0; i < in_size.size(); ++i)
+            if (n) LRB_CHECK(cudaMemcpyAsync(din[slot][i].get(), x[i], n * in_size[i], cudaMemcpyHostToDevice, s));
+        if (run(pin[slot].data(), n, pout[slot].data(), n_out, s) != 0) return -1;
+        for (size_t k = 0; k < out_size.size(); ++k)
+            if (n_out[k]) LRB_CHECK(cudaMemcpyAsync(y[k], pout[slot][k], n_out[k] * out_size[k], cudaMemcpyDeviceToHost, s));
+        return 0;
+    }
+
+    int ensure_pipeline() {
+        if (s_h2d) return 0;
+        LRB_CHECK(cudaStreamCreateWithFlags(&s_h2d, cudaStreamNonBlocking));
+        LRB_CHECK(cudaStreamCreateWithFlags(&s_d2h, cudaStreamNonBlocking));
+        for (int i = 0; i < 2; ++i) {
+            LRB_CHECK(cudaEventCreateWithFlags(&ev_h2d[i], cudaEventDisableTiming));
+            LRB_CHECK(cudaEventCreateWithFlags(&ev_comp[i], cudaEventDisableTiming));
+            LRB_CHECK(cudaEventCreateWithFlags(&ev_d2h[i], cudaEventDisableTiming));
+        }
+        return 0;
+    }
+
+    // host ins x[i] of n samples, host outs y[k] receiving n_out[k] samples -- or, in super-chunk mode, the vector appended
+    // to the current slot (y[k] then receives the outputs of the slots completed meanwhile)
+    int execute(const void* const* x, size_t n, void* const* y, size_t* n_out) {
+        if (samples) {
+            fed = true;
+            return accumulate((const char*)x[0], n, (char* const*)y, n_out);
+        }
+        cudaStream_t s = ctx().stream;
+        if (n <= chunk) {
+            if (reserve(0, n) != 0 || stage(0, x, n, y, n_out, s) != 0) return -1;
+            LRB_CHECK(cudaStreamSynchronize(s));
+            return 0;
+        }
+        if (ensure_pipeline() != 0) return -1;
+        std::vector<size_t> no(out_size.size());
+        for (size_t k = 0; k < out_size.size(); ++k) n_out[k] = 0;
+        for (size_t done_in = 0, it = 0; done_in < n; ++it) {
+            const int slot = (int)(it & 1);
+            const size_t nc = n - done_in < chunk ? n - done_in : chunk;
+            if (reserve(slot, nc) != 0) return -1;
+            if (it >= 2) LRB_CHECK(cudaStreamWaitEvent(s_h2d, ev_comp[slot], 0));     // the slot's inputs free again
+            for (size_t i = 0; i < in_size.size(); ++i)
+                LRB_CHECK(cudaMemcpyAsync(din[slot][i].get(), (const char*)x[i] + done_in * in_size[i], nc * in_size[i],
+                                          cudaMemcpyHostToDevice, s_h2d));
+            LRB_CHECK(cudaEventRecord(ev_h2d[slot], s_h2d));
+            LRB_CHECK(cudaStreamWaitEvent(s, ev_h2d[slot], 0));
+            if (it >= 2) LRB_CHECK(cudaStreamWaitEvent(s, ev_d2h[slot], 0));          // the slot's outputs drained
+            if (run(pin[slot].data(), nc, pout[slot].data(), no.data(), s) != 0) return -1;
+            LRB_CHECK(cudaEventRecord(ev_comp[slot], s));
+            LRB_CHECK(cudaStreamWaitEvent(s_d2h, ev_comp[slot], 0));
+            for (size_t k = 0; k < out_size.size(); ++k) {
+                if (no[k]) LRB_CHECK(cudaMemcpyAsync((char*)y[k] + n_out[k] * out_size[k], pout[slot][k], no[k] * out_size[k],
+                                                     cudaMemcpyDeviceToHost, s_d2h));
+                n_out[k] += no[k];
+            }
+            LRB_CHECK(cudaEventRecord(ev_d2h[slot], s_d2h));
+            done_in += nc;
+        }
+        // the last download is behind every upload and every run (event chain), so one synchronize drains all three
+        LRB_CHECK(cudaStreamSynchronize(s_d2h));
+        LRB_CHECK(cudaStreamSynchronize(s));     // (returns at once; keeps the compute stream's error state observable)
+        return 0;
+    }
+
+    // ---- super-chunk mode -----------------------------------------------------------------------------------------------
     void release() {
         for (int i = 0; i < 2; ++i) {
             hin[i].reset(); hout[i].clear();
-            din[i] = DeviceBuffer(); dout[i].clear();
             if (done[i]) cudaEventDestroy(done[i]);
             done[i] = nullptr;
             pending[i] = false; nout[i].clear();
         }
         samples = 0; fill = 0; cur = 0;
     }
-    // `cap[k]`: samples port k can produce from one slot of `samples` inputs
-    int configure(size_t n, size_t isz, const std::vector<size_t>& osz, const std::vector<size_t>& cap) {
+    // slots of n input samples (0: off), only while none is pending or partly filled
+    int set_superchunk(size_t n, const char* who) {
+        if (pending[0] || pending[1] || fill) { set_error("%s: flush before changing the super-chunk size", who); return -1; }
         release();
+        fed = false;
         if (n == 0) return 0;
-        in_size = isz; out_size = osz; outcap = cap;
+        outcap = max_out(n) + 1;
         for (int i = 0; i < 2; ++i) {
+            if (reserve(i, n) != 0) return -1;
             char* p = nullptr;
-            LRB_CHECK(cudaHostAlloc((void**)&p, n * isz, cudaHostAllocDefault));
+            LRB_CHECK(cudaHostAlloc((void**)&p, n * in_size[0], cudaHostAllocDefault));
             hin[i].reset(p);
-            if (din[i].reserve(n * isz) != 0) return -1;
-            hout[i].resize(ports());
-            dout[i].resize(ports());
-            nout[i].assign(ports(), 0);
-            for (size_t k = 0; k < ports(); ++k) {
-                LRB_CHECK(cudaHostAlloc((void**)&p, cap[k] * osz[k], cudaHostAllocDefault));
+            hout[i].resize(out_size.size());
+            nout[i].assign(out_size.size(), 0);
+            for (size_t k = 0; k < out_size.size(); ++k) {
+                LRB_CHECK(cudaHostAlloc((void**)&p, outcap * out_size[k], cudaHostAllocDefault));
                 hout[i][k].reset(p);
-                if (dout[i][k].reserve(cap[k] * osz[k]) != 0) return -1;
             }
             LRB_CHECK(cudaEventCreateWithFlags(&done[i], cudaEventDisableTiming));
         }
         samples = n;
         return 0;
     }
-    // wait for the slots in flight and forget them and the partial slot
+    // reset: wait for the slots in flight and forget them and the partial slot (the super-chunk size stays)
     int drop() {
         for (int i = 0; i < 2; ++i) {
             if (pending[i] && !cuda_ok(cudaEventSynchronize(done[i]), "cudaEventSynchronize")) return -1;
             pending[i] = false;
         }
-        fill = 0; cur = 0;
+        fill = 0; cur = 0; fed = false;
         return 0;
     }
     // append a finished slot's outputs to y[k] + produced[k]
     int collect(int slot, char* const* y, size_t* produced) {
         if (!pending[slot]) return 0;
         if (!cuda_ok(cudaEventSynchronize(done[slot]), "cudaEventSynchronize")) return -1;
-        for (size_t k = 0; k < ports(); ++k) {
+        for (size_t k = 0; k < out_size.size(); ++k) {
             if (nout[slot][k]) memcpy(y[k] + produced[k] * out_size[k], hout[slot][k].get(), nout[slot][k] * out_size[k]);
             produced[k] += nout[slot][k];
         }
         pending[slot] = false;
         return 0;
     }
-    int submit(int slot, size_t count, const Run& run) {
+    int submit(int slot, size_t count) {
         cudaStream_t s = ctx().stream;
-        std::vector<void*> dy(ports());
-        for (size_t k = 0; k < ports(); ++k) dy[k] = dout[slot][k].get();
-        LRB_CHECK(cudaMemcpyAsync(din[slot].get(), hin[slot].get(), count * in_size, cudaMemcpyHostToDevice, s));
-        if (run(din[slot].get(), count, dy.data(), nout[slot].data(), s) != 0) return -1;
-        for (size_t k = 0; k < ports(); ++k)
-            if (nout[slot][k])
-                LRB_CHECK(cudaMemcpyAsync(hout[slot][k].get(), dy[k], nout[slot][k] * out_size[k], cudaMemcpyDeviceToHost, s));
+        const void* hx = hin[slot].get();
+        std::vector<void*> hy(out_size.size());
+        for (size_t k = 0; k < out_size.size(); ++k) hy[k] = hout[slot][k].get();
+        if (stage(slot, &hx, count, hy.data(), nout[slot].data(), s) != 0) return -1;
         LRB_CHECK(cudaEventRecord(done[slot], s));
         pending[slot] = true;
         return 0;
     }
-    int accumulate(const void* x, size_t n, char* const* y, size_t* n_out, const Run& run) {
-        const char* xp = (const char*)x;
-        for (size_t k = 0; k < ports(); ++k) n_out[k] = 0;
+    int accumulate(const char* x, size_t n, char* const* y, size_t* n_out) {
+        for (size_t k = 0; k < out_size.size(); ++k) n_out[k] = 0;
         while (n > 0) {
             const size_t take = n < samples - fill ? n : samples - fill;
-            memcpy(hin[cur].get() + fill * in_size, xp, take * in_size);
-            fill += take; xp += take * in_size; n -= take;
+            memcpy(hin[cur].get() + fill * in_size[0], x, take * in_size[0]);
+            fill += take; x += take * in_size[0]; n -= take;
             if (fill == samples) {
                 // the other slot was submitted one super-chunk ago: its results are (long) ready
                 if (collect(cur ^ 1, y, n_out) != 0) return -1;
-                if (submit(cur, samples, run) != 0) return -1;
+                if (submit(cur, samples) != 0) return -1;
                 cur ^= 1;
                 fill = 0;
             }
         }
         return 0;
     }
-    int flush(char* const* y, size_t* n_out, const Run& run) {
-        for (size_t k = 0; k < ports(); ++k) n_out[k] = 0;
+    // the pending slot's outputs and the partial slot's; 0 samples when the mode is off
+    int flush(void* const* yv, size_t* n_out) {
+        char* const* y = (char* const*)yv;
+        for (size_t k = 0; k < out_size.size(); ++k) n_out[k] = 0;
+        fed = false;
         if (!samples) return 0;
         if (collect(cur ^ 1, y, n_out) != 0) return -1;
         if (fill) {
-            if (submit(cur, fill, run) != 0) return -1;
+            if (submit(cur, fill) != 0) return -1;
             if (collect(cur, y, n_out) != 0) return -1;
             fill = 0;
         }
         return 0;
     }
-    // room one call appending n samples may need in port k
-    size_t max_output(size_t k, size_t n) const { return (n / samples + 2) * outcap[k]; }
+    // a run past the boundary (device pointers, a shard) would overtake the samples waiting in the slots
+    int refuse_direct(const char* who, const char* what) const {
+        if (!samples) return 0;
+        set_error("%s: %s runs the stream directly; switch super-chunk mode off first (set_superchunk 0)", who, what);
+        return -1;
+    }
+    // room one host call of n inputs may need in any output port
+    size_t max_output(size_t n) const { return samples ? (n / samples + 2) * outcap : max_out(n); }
 };
+
+void HostBoundaryFree::operator()(HostBoundary* h) const { delete h; }
+
+static constexpr size_t HOST_CHUNK = (size_t)1 << 24;   // input samples per chunk of a host-mode block's call
+
+int Block::execute_multi(const void* const* x, int nin, size_t n, void* const* y, int nout, size_t* n_out) {
+    if (nin != num_inputs || nout != num_outputs) {
+        set_error("%s: expected %d input(s) and %d output(s), got %d and %d", name.c_str(), num_inputs, num_outputs, nin, nout);
+        return -1;
+    }
+    size_t produced = 0;
+    if (dev_ptrs) {
+        if (run_multi(x, nin, n, y, nout, &produced, ctx().stream) != 0) return -1;
+        if (n_out) *n_out = produced;
+        return 0;
+    }
+    if (!host) {
+        host.reset(new HostBoundary([this](const void* const* dx, size_t m, void* const* dy, size_t* no, cudaStream_t s) {
+            if (run_multi(dx, num_inputs, m, dy, num_outputs, no, s) != 0) return -1;
+            for (int o = 1; o < num_outputs; ++o) no[o] = no[0];      // every port produces the same count
+            return 0;
+        }, [this](size_t m) { return max_output(m); }, HOST_CHUNK));
+        host->in_size.assign((size_t)nin, in_size);
+        for (int o = 0; o < nout; ++o) host->out_size.push_back(out_size_of(o));
+    }
+    std::vector<size_t> counts((size_t)nout);
+    if (host->execute(x, n, y, counts.data()) != 0) return -1;
+    if (n_out) *n_out = counts[0];
+    return 0;
+}
 
 // ---- time-chunk sharding (SURVEY.md 8e): where a stream can be cut, for graphs and DAGs alike ---------------------------
 int Block::need_in(double need_out, double* need) const {
@@ -326,12 +473,6 @@ struct Graph : Block {
     std::vector<Block*> stages;      // execution order after commit (not owned)
     bool committed = false;
     DeviceBuffer ring[2];
-    // host-mode double buffering
-    DeviceBuffer d_in[2], d_out[2];
-    cudaStream_t s_h2d = nullptr, s_d2h = nullptr;
-    cudaEvent_t ev_h2d[2] = {nullptr, nullptr}, ev_comp[2] = {nullptr, nullptr}, ev_d2h[2] = {nullptr, nullptr};
-    size_t host_chunk = (size_t)1 << 23;   // input samples per pipelined chunk
-    SuperChunk sc;                   // super-chunk mode (lrb200_graph_set_superchunk)
     // time-chunk sharding (run_shard): scratch for the outputs that belong to the halo
     DeviceBuffer head_out;
     // optional per-stage timing
@@ -339,7 +480,20 @@ struct Graph : Block {
     std::vector<std::vector<cudaEvent_t>> tev;   // per stage: [start0, stop0, start1, stop1, ...]
     std::vector<int> tcount;
 
-    Graph() : Block("", 8, 8, true) {}      // element sizes and name (the description) are set by commit
+    // element sizes and name (the description) are set by commit; host calls go in chunks of 2^23 samples
+    Graph() : Block("", 8, 8, true) {
+        host.reset(new HostBoundary([this](const void* const* dx, size_t n, void* const* dy, size_t* n_out, cudaStream_t s) {
+            return run(dx[0], n, dy[0], n_out, s);
+        }, [this](size_t n) { return max_output(n); }, (size_t)1 << 23));
+    }
+    // the boundary of host calls and super-chunk mode, sized for the committed stages
+    HostBoundary* boundary() {
+        if (ensure_committed() != 0) return nullptr;
+        if (stages.empty()) { set_error("graph: no blocks"); return nullptr; }
+        host->in_size.assign(1, in_size);
+        host->out_size.assign(1, out_size);
+        return host.get();
+    }
 
     cudaEvent_t timing_event(size_t stage, size_t idx) {
         auto& v = tev[stage];
@@ -360,13 +514,6 @@ struct Graph : Block {
 
     ~Graph() override {
         for (auto& v : tev) for (cudaEvent_t e : v) cudaEventDestroy(e);
-        for (int i = 0; i < 2; ++i) {
-            if (ev_h2d[i]) cudaEventDestroy(ev_h2d[i]);
-            if (ev_comp[i]) cudaEventDestroy(ev_comp[i]);
-            if (ev_d2h[i]) cudaEventDestroy(ev_d2h[i]);
-        }
-        if (s_h2d) cudaStreamDestroy(s_h2d);
-        if (s_d2h) cudaStreamDestroy(s_d2h);
     }
 
     size_t max_output(size_t n) const override {
@@ -453,86 +600,6 @@ struct Graph : Block {
         return 0;
     }
 
-    int ensure_host_pipeline() {
-        if (s_h2d) return 0;
-        LRB_CHECK(cudaStreamCreateWithFlags(&s_h2d, cudaStreamNonBlocking));
-        LRB_CHECK(cudaStreamCreateWithFlags(&s_d2h, cudaStreamNonBlocking));
-        for (int i = 0; i < 2; ++i) {
-            LRB_CHECK(cudaEventCreateWithFlags(&ev_h2d[i], cudaEventDisableTiming));
-            LRB_CHECK(cudaEventCreateWithFlags(&ev_comp[i], cudaEventDisableTiming));
-            LRB_CHECK(cudaEventCreateWithFlags(&ev_d2h[i], cudaEventDisableTiming));
-        }
-        return 0;
-    }
-
-    // host in/out: pipelined H2D | kernels | D2H over two slots
-    int run_host(const void* x, size_t n, void* y, size_t* n_out) {
-        if (ensure_committed() != 0) return -1;
-        if (stages.empty()) { set_error("graph: no blocks"); return -1; }
-        cudaStream_t s = ctx().stream;
-        const size_t isz = in_size, osz = out_size;
-        if (sc.samples) return sc.accumulate(x, n, (char* const*)&y, n_out, sc_run());
-        if (n <= host_chunk) {
-            // one chunk (every call of the reference's per-vector regime, pipe.lua:73): copy, kernels and copy back in
-            // order on ONE stream with ONE synchronize -- no cross-stream events, nothing to overlap anyway
-            const size_t mo = max_output(n);
-            if (n * isz > d_in[0].capacity() || (mo ? mo : 1) * osz > d_out[0].capacity()) {
-                LRB_CHECK(cudaStreamSynchronize(s));
-                if (d_in[0].reserve((n ? n : 1) * isz) != 0 || d_out[0].reserve((mo ? mo : 1) * osz) != 0) return -1;
-            }
-            size_t no = 0;
-            if (n) LRB_CHECK(cudaMemcpyAsync(d_in[0].get(), x, n * isz, cudaMemcpyHostToDevice, s));
-            if (run(d_in[0].get(), n, d_out[0].get(), &no, s) != 0) return -1;
-            if (no) LRB_CHECK(cudaMemcpyAsync(y, d_out[0].get(), no * osz, cudaMemcpyDeviceToHost, s));
-            LRB_CHECK(cudaStreamSynchronize(s));
-            *n_out = no;
-            return 0;
-        }
-        if (ensure_host_pipeline() != 0) return -1;
-        size_t done = 0, produced = 0;
-        int it = 0;
-        while (done < n) {
-            const int slot = it & 1;
-            size_t nc = n - done < host_chunk ? n - done : host_chunk;
-            size_t mo = max_output(nc);
-            if (nc * isz > d_in[slot].capacity() || (mo ? mo : 1) * osz > d_out[slot].capacity()) {
-                LRB_CHECK(cudaDeviceSynchronize());
-                if (d_in[slot].reserve(nc * isz) != 0 || d_out[slot].reserve((mo ? mo : 1) * osz) != 0) return -1;
-            }
-            if (it >= 2) LRB_CHECK(cudaStreamWaitEvent(s_h2d, ev_comp[slot], 0));     // d_in[slot] free again
-            LRB_CHECK(cudaMemcpyAsync(d_in[slot].get(), (const char*)x + done * isz, nc * isz, cudaMemcpyHostToDevice, s_h2d));
-            LRB_CHECK(cudaEventRecord(ev_h2d[slot], s_h2d));
-            LRB_CHECK(cudaStreamWaitEvent(s, ev_h2d[slot], 0));
-            if (it >= 2) LRB_CHECK(cudaStreamWaitEvent(s, ev_d2h[slot], 0));          // d_out[slot] drained
-            size_t no = 0;
-            if (run(d_in[slot].get(), nc, d_out[slot].get(), &no, s) != 0) return -1;
-            LRB_CHECK(cudaEventRecord(ev_comp[slot], s));
-            LRB_CHECK(cudaStreamWaitEvent(s_d2h, ev_comp[slot], 0));
-            if (no) LRB_CHECK(cudaMemcpyAsync((char*)y + produced * osz, d_out[slot].get(), no * osz, cudaMemcpyDeviceToHost, s_d2h));
-            LRB_CHECK(cudaEventRecord(ev_d2h[slot], s_d2h));
-            produced += no;
-            done += nc;
-            ++it;
-        }
-        // the last download is behind every upload and every kernel (event chain), so one synchronize drains all three
-        LRB_CHECK(cudaStreamSynchronize(s_d2h));
-        LRB_CHECK(cudaStreamSynchronize(s));     // (returns at once; keeps the compute stream's error state observable)
-        *n_out = produced;
-        return 0;
-    }
-
-    // ---- super-chunk mode -------------------------------------------------------------------------------------
-    SuperChunk::Run sc_run() {
-        return [this](const void* dx, size_t n, void* const* dy, size_t* n_out, cudaStream_t s) { return run(dx, n, dy[0], n_out, s); };
-    }
-    int set_superchunk(size_t samples) {
-        if (ensure_committed() != 0) return -1;
-        if (stages.empty()) { set_error("graph: no blocks"); return -1; }
-        if (sc.busy()) { set_error("graph: flush before changing the super-chunk size"); return -1; }
-        return sc.configure(samples, in_size, {out_size}, {max_output(samples) + 1});
-    }
-    int flush(void* y, size_t* n_out) { return sc.flush((char* const*)&y, n_out, sc_run()); }
-
     // Block::reset for every block, with ONE launch zeroing the carried state of them all
     int reset(cudaStream_t s) {
         std::vector<void*> ptrs;
@@ -545,7 +612,7 @@ struct Graph : Block {
         if (ptrs.empty()) return 0;
         return launch_zero_segments(ptrs.data(), bytes.data(), (int)ptrs.size(), s);
     }
-    int reset() override { return reset(ctx().stream); }
+    int reset() override { return host->drop() != 0 ? -1 : reset(ctx().stream); }
 
     // ---- time-chunk sharding (SURVEY.md 8e) -------------------------------------------------------------------
     Rate total_rate() const {
@@ -660,9 +727,10 @@ struct Graph : Block {
 // every linear run).  Nodes are added in topological order; an input reference is (producer node, output port) or the
 // DAG's own input.  Every edge is a grow-only device buffer; all inputs of a node must deliver the same number of samples
 // per call (true whenever the converging paths have the same rate changes -- every block here is zero-latency; the
-// reference's PipeMux would buffer a surplus instead, radio/core/pipe.lua:495-615).  Host in, host out(s): one upload,
-// the node launches in order on the library stream, one download per output, one synchronize; or the same launches on
-// device-resident input and outputs with no synchronize; or host vectors packed into super-chunks (SuperChunk above).
+// reference's PipeMux would buffer a surplus instead, radio/core/pipe.lua:495-615).  Host in, host out(s) through the
+// HostBoundary above, a whole call as one chunk: one upload, the node launches in order on the library stream, one
+// download per output, one synchronize; or host vectors packed into super-chunks; or the same launches on device-resident
+// input and outputs with no synchronize.
 // This is what composites/wbfmstereodemodulator.lua:22-64 and amsynchronousdemodulator.lua:25-45 need on the device.
 // ---------------------------------------------------------------------------------------------------------------------
 // An output port of a node, or (node -1) the DAG's input.  The C ABI encodes it as node * 4 + port, or -1.
@@ -688,11 +756,21 @@ struct DagNode {
 struct Dag {
     std::vector<DagNode> nodes;
     std::vector<PortRef> outputs;  // never the DAG input
-    DeviceBuffer d_in;
     size_t in_size = 0;
     std::string desc;
-    SuperChunk sc;                 // super-chunk mode (lrb200_dag_set_superchunk)
-    bool sc_fed = false;           // an execute since super-chunk mode was set, or since the last flush / reset
+    // host calls and super-chunk mode; the run writes each output port straight into the boundary's staging
+    HostBoundary host{[this](const void* const* dx, size_t n, void* const* dy, size_t* n_out, cudaStream_t s) {
+        return run_nodes(dx[0], n, dy, n_out, s);
+    }, [this](size_t n) { return max_output(n); }, ~(size_t)0};
+
+    // the boundary, sized for the current input and output ports
+    HostBoundary* boundary() {
+        if (nodes.empty() || outputs.empty()) { set_error("dag: no nodes / no outputs"); return nullptr; }
+        host.in_size.assign(1, in_size);
+        host.out_size.resize(outputs.size());
+        for (size_t k = 0; k < outputs.size(); ++k) host.out_size[k] = out_size(k);
+        return &host;
+    }
 
     // on success the DAG owns blk; on failure the caller keeps it
     int add(Block* blk, const int* refs, unsigned nin) {
@@ -752,8 +830,7 @@ struct Dag {
     // back to the state after creation: the slots in flight are waited for and dropped with the partial slot (the
     // super-chunk size stays), then every node's carried state is zeroed
     int reset() {
-        if (sc.drop() != 0) return -1;
-        sc_fed = false;
+        if (host.drop() != 0) return -1;
         for (DagNode& nd : nodes)
             if (nd.blk->reset() != 0) return -1;
         return 0;
@@ -826,53 +903,6 @@ struct Dag {
         }
         for (int o = 0; o < nd.blk->num_outputs; ++o) nd.out_cnt[(size_t)o] = no;
         return 0;
-    }
-
-    SuperChunk::Run sc_run() {
-        return [this](const void* dx, size_t n, void* const* dy, size_t* n_out, cudaStream_t s) { return run_nodes(dx, n, dy, n_out, s); };
-    }
-
-    // host in, host outs: one upload, the node launches, one download per output, one synchronize -- or, in super-chunk
-    // mode, the vector appended to the current slot
-    int run_host(const void* x, size_t n, void* const* y, size_t* n_out) {
-        if (nodes.empty() || outputs.empty()) { set_error("dag: no nodes / no outputs"); return -1; }
-        if (sc.samples) {
-            sc_fed = true;
-            return sc.accumulate(x, n, (char* const*)y, n_out, sc_run());
-        }
-        cudaStream_t s = ctx().stream;
-        if (n * in_size > d_in.capacity()) {
-            LRB_CHECK(cudaStreamSynchronize(s));
-            if (d_in.reserve(n * in_size) != 0) return -1;
-        }
-        if (n) LRB_CHECK(cudaMemcpyAsync(d_in.get(), x, n * in_size, cudaMemcpyHostToDevice, s));
-        if (run_nodes(d_in.get(), n, nullptr, n_out, s) != 0) return -1;
-        for (size_t k = 0; k < outputs.size(); ++k)
-            if (n_out[k]) LRB_CHECK(cudaMemcpyAsync(y[k], port_ptr(outputs[k], nullptr), n_out[k] * out_size(k), cudaMemcpyDeviceToHost, s));
-        LRB_CHECK(cudaStreamSynchronize(s));
-        return 0;
-    }
-
-    int run_device(const void* dx, size_t n, void* const* dy, size_t* n_out) {
-        if (sc.samples) { set_error("dag: execute_device runs the stream directly; switch super-chunk mode off first (set_superchunk 0)"); return -1; }
-        return run_nodes(dx, n, dy, n_out, ctx().stream);
-    }
-
-    int set_superchunk(size_t samples) {
-        if (nodes.empty() || outputs.empty()) { set_error("dag: no nodes / no outputs"); return -1; }
-        if (sc.busy()) { set_error("dag: flush before changing the super-chunk size"); return -1; }
-        std::vector<size_t> osz, cap;
-        for (size_t k = 0; k < outputs.size(); ++k) { osz.push_back(out_size(k)); cap.push_back(max_output(samples) + 1); }
-        sc_fed = false;
-        return sc.configure(samples, in_size, osz, cap);
-    }
-
-    int flush(void* const* y, size_t* n_out) {
-        for (size_t k = 0; k < outputs.size(); ++k) n_out[k] = 0;
-        if (!sc.samples) { set_error("dag: flush needs super-chunk mode (set_superchunk)"); return -1; }
-        if (!sc_fed) { set_error("dag: nothing to flush: no execute since super-chunk mode was set, the last flush or reset"); return -1; }
-        sc_fed = false;
-        return sc.flush((char* const*)y, n_out, sc_run());
     }
 
     // ---- time-chunk sharding (SURVEY.md 8e) ---------------------------------------------------------------------------
@@ -981,8 +1011,7 @@ struct Dag {
 
     int shard_begin(const void* dx, size_t halo_n, size_t n, uint64_t start, void* const* dy, size_t* n_out, void* record,
                     size_t record_bytes_) {
-        if (sc.samples) { set_error("dag: sharding runs the stream directly; switch super-chunk mode off first (set_superchunk 0)"); return -1; }
-        if (plan() != 0 || check_record(record_bytes_) != 0) return -1;
+        if (host.refuse_direct("dag", "sharding") != 0 || plan() != 0 || check_record(record_bytes_) != 0) return -1;
         bool first;
         if (shard_args("dag", halo_n, start, sh.period, &first) != 0) return -1;
         sh.pending = false;
@@ -1149,7 +1178,8 @@ int lrb200_graph_commit(lrb200_graph_t* g, int fuse) {
 int lrb200_graph_execute(lrb200_graph_t* g, const void* x, size_t n, void* y, size_t* n_out) {
     if (!g) { set_error("null graph"); return -1; }
     size_t no = 0;
-    int rc = g->g->run_host(x, n, y, &no);
+    HostBoundary* hb = g->g->boundary();
+    int rc = hb ? hb->execute(&x, n, &y, &no) : -1;
     if (n_out) *n_out = no;
     return rc;
 }
@@ -1157,7 +1187,7 @@ int lrb200_graph_execute(lrb200_graph_t* g, const void* x, size_t n, void* y, si
 int lrb200_graph_execute_device(lrb200_graph_t* g, const void* dx, size_t n, void* dy, size_t* n_out) {
     if (!g) { set_error("null graph"); return -1; }
     size_t no = 0;
-    int rc = g->g->run(dx, n, dy, &no, ctx().stream);
+    int rc = g->g->host->refuse_direct("graph", "execute_device") != 0 ? -1 : g->g->run(dx, n, dy, &no, ctx().stream);
     if (n_out) *n_out = no;
     return rc;
 }
@@ -1167,19 +1197,19 @@ size_t lrb200_graph_max_output(const lrb200_graph_t* g, size_t n) {
     Graph& gr = *g->g;
     if (gr.ensure_committed() != 0) return 0;
     // super-chunk mode: one call may hand back the results of the slots completed while n samples were appended
-    if (gr.sc.samples) return gr.sc.max_output(0, n);
-    return gr.max_output(n);
+    return gr.host->max_output(n);
 }
 
 int lrb200_graph_set_superchunk(lrb200_graph_t* g, size_t samples) {
     if (!g) { set_error("null graph"); return -1; }
-    return g->g->set_superchunk(samples);
+    HostBoundary* hb = g->g->boundary();
+    return hb ? hb->set_superchunk(samples, "graph") : -1;
 }
 
 int lrb200_graph_flush(lrb200_graph_t* g, void* y, size_t* n_out) {
     if (!g) { set_error("null graph"); return -1; }
     size_t no = 0;
-    int rc = g->g->flush(y, &no);
+    int rc = g->g->host->flush(&y, &no);     // 0 samples with super-chunk mode off or nothing fed
     if (n_out) *n_out = no;
     return rc;
 }
@@ -1194,7 +1224,7 @@ int lrb200_graph_execute_shard(lrb200_graph_t* g, lrb200_graph_t* g_head, const 
     if (!g) { set_error("null graph"); return -1; }
     size_t no = 0;
     (void)g_head;
-    int rc = g->g->run_shard(dx, halo, n, start, dy, &no, (cudaEvent_t)halo_ready_event);
+    int rc = g->g->host->refuse_direct("graph", "sharding") != 0 ? -1 : g->g->run_shard(dx, halo, n, start, dy, &no, (cudaEvent_t)halo_ready_event);
     if (n_out) *n_out = no;
     return rc;
 }
@@ -1284,7 +1314,7 @@ int lrb200_dag_add_graph(lrb200_dag_t* d, lrb200_graph_t* g, int input) {
 
 int lrb200_dag_set_outputs(lrb200_dag_t* d, const int* outputs, unsigned num_outputs) {
     if (!d || !outputs || !num_outputs) { set_error("dag_set_outputs: null argument"); return -1; }
-    if (d->d.sc.samples) { set_error("dag_set_outputs: the super-chunk slots are sized for the outputs; set them first"); return -1; }
+    if (d->d.host.samples) { set_error("dag_set_outputs: the super-chunk slots are sized for the outputs; set them first"); return -1; }
     std::vector<PortRef> refs(num_outputs);
     for (unsigned k = 0; k < num_outputs; ++k)
         if (d->d.decode(outputs[k], &refs[k]) != 0) { set_error("dag_set_outputs: bad reference %d", outputs[k]); return -1; }
@@ -1295,29 +1325,35 @@ int lrb200_dag_set_outputs(lrb200_dag_t* d, const int* outputs, unsigned num_out
 
 int lrb200_dag_execute(lrb200_dag_t* d, const void* x, size_t n, void* const* y, size_t* n_out) {
     if (!d || !y || !n_out || (n && !x)) { set_error("dag_execute: null argument"); return -1; }
-    return d->d.run_host(x, n, y, n_out);
+    HostBoundary* hb = d->d.boundary();
+    return hb ? hb->execute(&x, n, y, n_out) : -1;
 }
 
 int lrb200_dag_execute_device(lrb200_dag_t* d, const void* dx, size_t n, void* const* dy, size_t* n_out) {
     if (!d || !dy || !n_out || (n && !dx)) { set_error("dag_execute_device: null argument"); return -1; }
-    return d->d.run_device(dx, n, dy, n_out);
+    if (d->d.host.refuse_direct("dag", "execute_device") != 0) return -1;
+    return d->d.run_nodes(dx, n, dy, n_out, ctx().stream);
 }
 
 size_t lrb200_dag_max_output(const lrb200_dag_t* d, unsigned output, size_t n) {
     if (!d || output >= d->d.outputs.size()) return 0;
     // super-chunk mode: one call may hand back the results of the slots completed while n samples were appended
-    if (d->d.sc.samples) return d->d.sc.max_output(output, n);
-    return d->d.max_output(n);
+    return d->d.host.max_output(n);
 }
 
 int lrb200_dag_set_superchunk(lrb200_dag_t* d, size_t samples) {
     if (!d) { set_error("null dag"); return -1; }
-    return d->d.set_superchunk(samples);
+    HostBoundary* hb = d->d.boundary();
+    return hb ? hb->set_superchunk(samples, "dag") : -1;
 }
 
 int lrb200_dag_flush(lrb200_dag_t* d, void* const* y, size_t* n_out) {
     if (!d || !y || !n_out) { set_error("dag_flush: null argument"); return -1; }
-    return d->d.flush(y, n_out);
+    HostBoundary& hb = d->d.host;
+    for (size_t k = 0; k < d->d.outputs.size(); ++k) n_out[k] = 0;
+    if (!hb.samples) { set_error("dag: flush needs super-chunk mode (set_superchunk)"); return -1; }
+    if (!hb.fed) { set_error("dag: nothing to flush: no execute since super-chunk mode was set, the last flush or reset"); return -1; }
+    return hb.flush(y, n_out);
 }
 
 int lrb200_dag_reset(lrb200_dag_t* d) {
