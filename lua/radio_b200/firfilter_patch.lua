@@ -1,8 +1,8 @@
 ---
 -- FIRFilterBlock on the H100: the extra branch a maintainer adds at the TOP of the backend ladder in
 -- radio/blocks/signal/firfilter.lua (:88 `if platform.features.volk then`), mechanically identical to
--- the liquid branch (:165-226).  Lowpass/Highpass/Bandpass/Bandstop/ComplexBandpass/ComplexBandstop
--- inherit it unchanged because they only design taps and call FIRFilterBlock.initialize.
+-- the liquid branch (:165-226).  Lowpass/Highpass/Bandpass/Bandstop/ComplexBandpass/ComplexBandstop, RootRaisedCosine
+-- and ManchesterMatchedFilter inherit it unchanged because they only design taps and call FIRFilterBlock.initialize.
 --
 --   if platform.features.cuda then  <this file's body>  elseif platform.features.volk then ...
 

@@ -25,7 +25,8 @@ from .signal_blocks import (MultiplyConstantBlock, UpsamplerBlock, BandpassFilte
                             HighpassFilterBlock, HilbertTransformBlock, IIRFilterBlock, LowpassFilterBlock,
                             SinglepoleHighpassFilterBlock, SinglepoleLowpassFilterBlock,
                             MultiplyBlock, MultiplyConjugateBlock, AddBlock, SubtractBlock, DelayBlock, PLLBlock, GPUMultiBlock,
-                            AGCBlock, PowerSquelchBlock, RootRaisedCosineFilterBlock, BinaryPhaseCorrectorBlock)
+                            AGCBlock, PowerSquelchBlock, RootRaisedCosineFilterBlock, BinaryPhaseCorrectorBlock,
+                            ManchesterMatchedFilterBlock)
 from .types import ComplexFloat32, Float32, Vector
 from .utilities import filter_utils, spectrum_utils, window_utils
 

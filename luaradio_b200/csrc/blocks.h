@@ -113,7 +113,8 @@ inline long long decay_samples(double c) {        // samples until |c|^k < 1e-12
 constexpr int FIR_FFT_N = 1024;
 constexpr int FFT_MAX_TAPS = 513;       // L >= 512: at most half of every block is overlap
 struct FirFast {
-    int in_mode = 0;           // 0: complex in; 1: real in, two blocks packed per transform (rrrf); 2: Hilbert
+    int in_mode = 0;           // 0: complex in; 1: real in, two blocks packed per transform (rrrf); 2: Hilbert;
+                               // 3: complex in, magnitude at the load, then as 1
     int M = 0, D = 1;
     int nparts = 1;            // > 1: uniformly partitioned overlap-save for filters longer than one block allows
     int part_taps = 0;         // taps per partition (M unless partitioned)
@@ -124,7 +125,7 @@ struct FirFast {
     DeviceBuffer d_E;
     int block_len() const { return FIR_FFT_N - (part_taps - 1); }     // L: outputs per block
 };
-int fir_fast_prepare(FirKind kind, const void* taps, int M, int D, bool rotate, uint64_t rot_fix,
+int fir_fast_prepare(FirKind kind, const void* taps, int M, int D, bool rotate, uint64_t rot_fix, bool magnitude,
                      std::unique_ptr<FirFast>* out);
 int launch_overlap_save(const FirFast& f, const void* x, const void* hist, long long n, void* y, long long first,
                         uint64_t g0, cudaStream_t s);
@@ -146,6 +147,7 @@ struct FirBlock : Block {
     int cur = 0;
     int algo = 0;                     // LRB200_FIR_AUTO / DIRECT / FFT
     bool rotate = false;              // fused FrequencyTranslator in front (graph fusion; FFT path only)
+    bool magnitude = false;           // fused ComplexMagnitude in front: complex in, rrrf taps (graph fusion; FFT path only)
     double rot_turns = 0.0;
     uint64_t rot_fix = 0;
     // the kernels that cover this block, decided at init: overlap-save plan, polyphase taps, generic polyphase shape
@@ -159,9 +161,10 @@ struct FirBlock : Block {
     int pcur = 0;
     int set_pole(float c);
 
-    // rotate: a FrequencyTranslator of turns_per_sample fused in front (graph fusion)
+    // rotate: a FrequencyTranslator of turns_per_sample fused in front; magnitude: a ComplexMagnitude fused in front of
+    // real taps (graph fusion)
     FirBlock(FirKind k, const void* taps_host, unsigned ntaps, unsigned decim, bool dev, bool rotate = false,
-             double turns_per_sample = 0.0);
+             double turns_per_sample = 0.0, bool magnitude = false);
     ~FirBlock() override;
     int init() override;
     size_t max_output(size_t n) const override;

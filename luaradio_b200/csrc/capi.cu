@@ -85,11 +85,14 @@ int Block::reset() {
 // ---------------------------------------------------------------------------------------------
 // FIR (+ Hilbert)
 // ---------------------------------------------------------------------------------------------
-FirBlock::FirBlock(FirKind k, const void* taps_host, unsigned ntaps, unsigned decim, bool dev, bool rot, double turns_per_sample)
+FirBlock::FirBlock(FirKind k, const void* taps_host, unsigned ntaps, unsigned decim, bool dev, bool rot, double turns_per_sample,
+                   bool mag)
     : Block(rot ? (k == FIR_CCCF ? "rot+fir_cccf" : "rot+fir_crcf")
+                : mag ? "mag+fir_rrrf"
                 : (k == FIR_CRCF ? "fir_crcf" : k == FIR_CCCF ? "fir_cccf" : k == FIR_RRRF ? "fir_rrrf" : "hilbert"),
-            (k == FIR_CRCF || k == FIR_CCCF) ? 8 : 4, k == FIR_RRRF ? 4 : 8, dev) {
+            (k == FIR_CRCF || k == FIR_CCCF || mag) ? 8 : 4, k == FIR_RRRF ? 4 : 8, dev) {
     kind = k;
+    magnitude = mag;
     M = (int)ntaps;
     D = (int)decim;
     tap_size = (k == FIR_CCCF) ? 8 : 4;
@@ -106,11 +109,13 @@ int FirBlock::init() {
     if (d_taps.upload(h_taps.data(), (size_t)M * tap_size) != 0) return -1;
     if (carry(d_hist, (size_t)(M > 1 ? M - 1 : 1) * in_size, cur) != 0) return -1;
     // register-tiled direct kernel: decimators with <= 128 taps and plain FIRs with <= 32 taps (complex in, real taps)
+    // (the fused magnitude exists only in the overlap-save kernel: no direct kernel is prepared for it)
     if (kind == FIR_CRCF && !rotate) poly = polyphase_prepare((const float*)h_taps.data(), M, D, 0.0);
-    if (kind == FIR_RRRF && D > 1) poly = polyphase_prepare((const float*)h_taps.data(), M, D, 0.0, false, true);
-    gen_poly = !rotate && D >= 2 && poly_generic_supports(kind, M, D);
-    if (fir_fast_prepare(kind, h_taps.data(), M, D, rotate, rot_fix, &fast) != 0) return -1;
+    if (kind == FIR_RRRF && D > 1 && !magnitude) poly = polyphase_prepare((const float*)h_taps.data(), M, D, 0.0, false, true);
+    gen_poly = !rotate && !magnitude && D >= 2 && poly_generic_supports(kind, M, D);
+    if (fir_fast_prepare(kind, h_taps.data(), M, D, rotate, rot_fix, magnitude, &fast) != 0) return -1;
     if (rotate && !fast) { set_error("fir: fused translator needs the overlap-save path (ntaps <= %d)", FFT_MAX_TAPS); return -1; }
+    if (magnitude && !fast) { set_error("fir: fused magnitude needs the overlap-save path (real taps, ntaps <= %d)", FFT_MAX_TAPS); return -1; }
     return 0;
 }
 
@@ -158,14 +163,16 @@ static bool overlap_save_cheaper(const FirBlock& f) {
     return direct_cost > fft_cost;
 }
 
-// Which kernel runs a call: tests/fft_fir_ref.py FirModel.plan states the same choices.
+// Which kernel runs a call: tests/fft_fir_ref.py FirModel.plan states the same choices (tests/ert_ref.py MagFirModel for
+// the fused magnitude).
 FirPath FirBlock::path(size_t n) const {
     if (always_polyphase()) return FirPath::Polyphase;
-    // the fused translator exists only in the overlap-save kernel (init refuses a rotating FIR without the plan)
-    const bool fft = rotate || (fast && (algo == LRB200_FIR_FFT || (algo == LRB200_FIR_AUTO && overlap_save_cheaper(*this))));
+    // the fused translator and magnitude exist only in the overlap-save kernel (init refuses such a FIR without the plan)
+    const bool fused_in = rotate || magnitude;
+    const bool fft = fused_in || (fast && (algo == LRB200_FIR_FFT || (algo == LRB200_FIR_AUTO && overlap_save_cheaper(*this))));
     if (!fft) return gen_poly ? FirPath::PolyGeneric : FirPath::Direct;
-    // a forced FFT (or a fused translator) always runs; the automatic choice leaves short calls to the catch-all
-    if (algo != LRB200_FIR_FFT && !rotate && n < 8 * (size_t)fast->block_len()) return FirPath::Direct;
+    // a forced FFT (or a fused translator or magnitude) always runs; the automatic choice leaves short calls to the catch-all
+    if (algo != LRB200_FIR_FFT && !fused_in && n < 8 * (size_t)fast->block_len()) return FirPath::Direct;
     return fast->nparts > 1 ? FirPath::DelayLine : FirPath::OverlapSave;
 }
 

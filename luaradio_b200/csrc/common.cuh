@@ -164,6 +164,9 @@ __device__ __forceinline__ float2 ffma2(float2 a, float2 b, float2 c) {
 __device__ __forceinline__ float2 fmul2(float2 a, float2 b) { return make_float2(__fmul_rn(a.x, b.x), __fmul_rn(a.y, b.y)); }
 __device__ __forceinline__ float2 fadd2(float2 a, float2 b) { return make_float2(__fadd_rn(a.x, b.x), __fadd_rn(a.y, b.y)); }
 __device__ __forceinline__ float2 fsub2(float2 a, float2 b) { return make_float2(__fsub_rn(a.x, b.x), __fsub_rn(a.y, b.y)); }
+// |v| as ComplexMagnitudeBlock computes it (complexmagnitude.lua:28-36): sqrt(re*re + im*im), one FMA, correctly rounded
+// square root.  The magnitude kernel and the overlap-save FIR's magnitude prologue both use it, so they agree bit for bit.
+__device__ __forceinline__ float cmag_of(float2 v) { return __fsqrt_rn(__fmaf_rn(v.x, v.x, __fmul_rn(v.y, v.y))); }
 // exp(j*2*pi*turns) for turns given as a 64-bit fixed-point fraction of a cycle.
 __device__ __forceinline__ float2 phasor_from_fix(uint64_t ph) {
     // top 32 bits as a signed fraction of a half-turn: t in [-1, 1)

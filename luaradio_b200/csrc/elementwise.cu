@@ -105,16 +105,16 @@ cmag_kernel(const float2* __restrict__ x, float* __restrict__ y, long long n, in
         for (; p < nquads; p += stride) {
             float4 a = __ldcs(x4 + 2 * p), b = __ldcs(x4 + 2 * p + 1);
             float4 o;
-            o.x = sqrtf(fmaf(a.x, a.x, a.y * a.y));
-            o.y = sqrtf(fmaf(a.z, a.z, a.w * a.w));
-            o.z = sqrtf(fmaf(b.x, b.x, b.y * b.y));
-            o.w = sqrtf(fmaf(b.z, b.z, b.w * b.w));
+            o.x = cmag_of(make_float2(a.x, a.y));
+            o.y = cmag_of(make_float2(a.z, a.w));
+            o.z = cmag_of(make_float2(b.x, b.y));
+            o.w = cmag_of(make_float2(b.z, b.w));
             __stcs(y4 + p, o);
         }
         long long i = (nquads << 2) + (long long)blockIdx.x * blockDim.x + threadIdx.x;
-        if (i < n) { float2 v = x[i]; y[i] = sqrtf(fmaf(v.x, v.x, v.y * v.y)); }
+        if (i < n) y[i] = cmag_of(x[i]);
     } else {
-        for (; p < n; p += stride) { float2 v = x[p]; y[p] = sqrtf(fmaf(v.x, v.x, v.y * v.y)); }
+        for (; p < n; p += stride) y[p] = cmag_of(x[p]);
     }
 }
 

@@ -28,6 +28,7 @@
 #include <cmath>
 #include <complex>
 #include <new>
+#include <type_traits>
 #include <vector>
 
 namespace lrb {
@@ -39,6 +40,7 @@ constexpr int FF_WARPS = 8;                       // warps (= concurrent FFT blo
 constexpr int FF_THREADS = FF_WARPS * 32;
 constexpr int FF_XSTRIDE = 33;                    // padded row stride of the transpose tile (float2 units)
 constexpr int FF_XCH = 32 * FF_XSTRIDE;           // float2 per warp-private tile
+constexpr int FF_MAG_BATCH = 8;                   // IN 3: complex samples per block loaded ahead of their magnitudes
 
 __device__ __forceinline__ float2 cmul_conj_if(float2 a, float2 w, bool conj) {
     // a * w  or  a * conj(w)
@@ -61,6 +63,10 @@ struct FftArgs {
     int M, D;
 };
 
+// a real input sample of the packed-real modes: IN 1 reads it, IN 3 takes the magnitude of a complex sample
+__device__ __forceinline__ float real_in(float a) { return a; }
+__device__ __forceinline__ float real_in(float2 a) { return cmag_of(a); }
+
 // floor division helpers for (possibly negative) t and positive d
 __device__ __forceinline__ void floor_divmod(long long t, int d, long long* q, int* r) {
     long long qq = t / d;
@@ -72,6 +78,7 @@ __device__ __forceinline__ void floor_divmod(long long t, int d, long long* q, i
 
 // IN   0: complex in / complex out (crcf, cccf)         1: real in, two blocks packed per FFT / real out (rrrf)
 //      2: real in / complex out with complex taps (Hilbert: taps = delay + j*hilbert)
+//      3: complex in, |x| taken at the load (fused ComplexMagnitude), then as IN 1: real taps, real out
 // EDGE false: interior blocks [b_lo, b_hi): all N inputs inside x, unconditional coalesced loads (one code path:
 //             guarded loads made the compiler clone the butterfly networks behind each branch);
 //      true : blocks touching the carried history (b = 0) or the end of the input (b >= b_hi), bounds-checked;
@@ -126,19 +133,34 @@ fir_fft1024_kernel(const __grid_constant__ FftArgs A) {
 #pragma unroll
                 for (int r = 0; r < 32; ++r) v[r] = cmul_conj_if(v[r], s_E[r * 32 + lane], false);
             }
-        } else if constexpr (IN == 1) {
-            // two consecutive real blocks 2b, 2b+1 as real / imaginary part
-            const float* x = reinterpret_cast<const float*>(A.x);
-            const float* hist = reinterpret_cast<const float*>(A.hist);
+        } else if constexpr (IN == 1 || IN == 3) {
+            // two consecutive real blocks 2b, 2b+1 as real / imaginary part (IN 3: the history holds complex samples too)
+            using T = typename std::conditional<IN == 3, float2, float>::type;
+            const T* x = reinterpret_cast<const T*>(A.x);
+            const T* hist = reinterpret_cast<const T*>(A.hist);
             const long long base0 = (2 * b) * L - Hm1, base1 = base0 + L;
+            T ld0[FF_MAG_BATCH], ld1[FF_MAG_BATCH];
+            (void)ld0; (void)ld1;
 #pragma unroll
             for (int r = 0; r < 32; ++r) {
                 const long long i0 = base0 + 32 * r + lane, i1 = base1 + 32 * r + lane;
-                if constexpr (!EDGE) {
-                    v[r] = make_float2(__ldcs(x + i0), __ldcs(x + i1));
+                if constexpr (!EDGE && IN == 3) {
+                    // the correctly rounded square root has a slow-path branch the compiler does not move loads across:
+                    // issue a batch of loads ahead of its magnitudes so that they are in flight together
+                    if (r % FF_MAG_BATCH == 0) {
+#pragma unroll
+                        for (int j = 0; j < FF_MAG_BATCH; ++j) {
+                            ld0[j] = __ldcs(x + i0 + 32 * j);
+                            ld1[j] = __ldcs(x + i1 + 32 * j);
+                        }
+                    }
+                    v[r] = make_float2(real_in(ld0[r % FF_MAG_BATCH]), real_in(ld1[r % FF_MAG_BATCH]));
+                } else if constexpr (!EDGE) {
+                    v[r] = make_float2(real_in(__ldcs(x + i0)), real_in(__ldcs(x + i1)));
                 } else {
-                    const float a = (i0 >= 0) ? (i0 < n ? __ldg(x + i0) : 0.f) : __ldg(hist + (Hm1 + i0));
-                    const float c = (i1 >= 0) ? (i1 < n ? __ldg(x + i1) : 0.f) : ((Hm1 + i1 >= 0) ? __ldg(hist + (Hm1 + i1)) : 0.f);
+                    const float a = (i0 >= 0) ? (i0 < n ? real_in(__ldg(x + i0)) : 0.f) : real_in(__ldg(hist + (Hm1 + i0)));
+                    const float c = (i1 >= 0) ? (i1 < n ? real_in(__ldg(x + i1)) : 0.f)
+                                              : ((Hm1 + i1 >= 0) ? real_in(__ldg(hist + (Hm1 + i1))) : 0.f);
                     v[r] = make_float2(a, c);
                 }
             }
@@ -528,15 +550,16 @@ int launch_fdl(const FdlArgs& a, cudaStream_t s) {
 // Host-side plan: tap spectrum (float64 DFT of the zero-extended taps, scaled by 1/N, as
 // firfilter.lua:337-343 does with spectrum_utils.DFT) and the 32x32 inter-pass twiddle table.
 // ---------------------------------------------------------------------------------------------
-int fir_fast_prepare(FirKind kind, const void* taps, int M, int D, bool rotate, uint64_t rot_fix,
+int fir_fast_prepare(FirKind kind, const void* taps, int M, int D, bool rotate, uint64_t rot_fix, bool magnitude,
                      std::unique_ptr<FirFast>* out) {
     if (kind == FIR_HILBERT && D != 1) return 0;
+    if (magnitude && kind != FIR_RRRF) return 0;
     const bool long_filter = M > FFT_MAX_TAPS;
     // long filters: complex-input, no fused decimation/translator -> P partitions of 512 taps, P passes over x
     if (long_filter && !((kind == FIR_CRCF || kind == FIR_CCCF) && D == 1 && !rotate && M <= 16 * 512)) return 0;
     std::unique_ptr<FirFast> fast(new (std::nothrow) FirFast());
     if (!fast) { set_error("out of memory"); return -1; }
-    fast->in_mode = (kind == FIR_RRRF) ? 1 : (kind == FIR_HILBERT ? 2 : 0);
+    fast->in_mode = magnitude ? 3 : (kind == FIR_RRRF) ? 1 : (kind == FIR_HILBERT ? 2 : 0);
     fast->M = M;
     fast->D = D;
     fast->part_taps = long_filter ? 512 : M;
@@ -610,7 +633,7 @@ int launch_overlap_save(const FirFast& f, const void* x, const void* hist, long 
                         uint64_t g0, cudaStream_t s) {
     const int L = f.block_len();
     // blocks of L outputs; in packed-real mode one FFT covers two of them
-    const long long per = (f.in_mode == 1) ? 2LL * L : (long long)L;
+    const long long per = (f.in_mode == 1 || f.in_mode == 3) ? 2LL * L : (long long)L;
     const long long nblocks = (n + per - 1) / per;
     // interior blocks [b_lo, b_hi): b*per - (M-1) >= 0  and  (b+1)*per <= n
     long long b_lo = ((long long)(f.M - 1) + per - 1) / per;
@@ -632,6 +655,7 @@ int launch_overlap_save(const FirFast& f, const void* x, const void* hist, long 
             return dec ? launch_fft<0, false, true>(a, n_int, n_edge, s) : launch_fft<0, false, false>(a, n_int, n_edge, s);
         case 1:
             return dec ? launch_fft<1, false, true>(a, n_int, n_edge, s) : launch_fft<1, false, false>(a, n_int, n_edge, s);
+        case 3: return launch_fft<3, false, true>(a, n_int, n_edge, s);     // the fused magnitude decimates (D may be 1)
         default:
             return launch_fft<2, false, false>(a, n_int, n_edge, s);
     }

@@ -136,6 +136,29 @@ static int fuse_noble_identity(const Blocks& blocks, size_t i, Rewrite* out) {
     return 0;
 }
 
+// ComplexMagnitude -> FIR(rrrf, D = 1) -> Downsampler(4 B, D > 1), or ComplexMagnitude -> FIR(rrrf, D > 1)  =>  overlap-save
+// FIR that takes |x| at its load (the ERT receiver's front end, composites/ertreceiver.lua:38-43).  The magnitude stream
+// never goes through HBM: 8 B read per input sample instead of 8 + 4 + 4.  No match for an undecimated FIR, or where the
+// decimating FIR fuse_fir_decimator would make does not run the overlap-save kernel on long calls (a polyphase shape, a
+// forced direct form, taps the single-block plan does not cover): those keep their own kernel choice.
+static int fuse_magnitude_fir(const Blocks& blocks, size_t i, Rewrite* out) {
+    C2fBlock* mag = block_at<C2fBlock>(blocks, i);
+    FirBlock* fir = block_at<FirBlock>(blocks, i + 1);
+    if (!mag || mag->op != 0 || !fir || fir->kind != FIR_RRRF || fir->rotate || fir->magnitude || fir->has_pole) return 0;
+    DownsampleBlock* down = fir->D == 1 ? block_at<DownsampleBlock>(blocks, i + 2) : nullptr;
+    if (down && down->in_size != 4) down = nullptr;
+    const int D = fir->D * (down ? down->D : 1);
+    if (D <= 1) return 0;
+    auto plain = make_block<FirBlock>(FIR_RRRF, fir->h_taps.data(), (unsigned)fir->M, (unsigned)D, true);
+    if (!plain) return -1;
+    if (plain->set_algorithm(fir->algo) != 0) return -1;
+    if (plain->effective_algorithm() != LRB200_FIR_FFT) return 0;
+    out->stage = make_block<FirBlock>(FIR_RRRF, fir->h_taps.data(), (unsigned)fir->M, (unsigned)D, true, false, 0.0, true);
+    if (!out->stage) return -1;
+    out->used = down ? 3 : 2;
+    return 0;
+}
+
 // FIR(D = 1, not Hilbert) -> Downsampler(D)  =>  decimating FIR (composites/decimator.lua:34-41)
 static int fuse_fir_decimator(const Blocks& blocks, size_t i, Rewrite* out) {
     FirBlock* fir = block_at<FirBlock>(blocks, i);
@@ -165,7 +188,7 @@ static int fuse_iir_decimator(const Blocks& blocks, size_t i, Rewrite* out) {
 
 // in priority order: the first rule that matches at a block wins
 static const Rule FUSION_RULES[] = {fuse_tuner, fuse_rotator_overlap_save, fuse_interpolator, fuse_noble_identity,
-                                   fuse_fir_decimator, fuse_iir_decimator};
+                                   fuse_magnitude_fir, fuse_fir_decimator, fuse_iir_decimator};
 
 // The host <-> device boundary of a device run: a linear graph, a device DAG, or a block created without LRB200_DEVICE.
 // The owner gives its run, a bound on a run's outputs per port, its ports' element sizes and its chunk length.  A host

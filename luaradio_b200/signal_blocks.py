@@ -550,6 +550,31 @@ class RootRaisedCosineFilterBlock(FIRFilterBlock):
         FIRFilterBlock.initialize(self)
 
 
+class ManchesterMatchedFilterBlock(FIRFilterBlock):
+    """manchestermatchedfilter.lua:27-51: an FIR filter matched to a Manchester-coded symbol, floor(rate / baudrate) taps of
+    -1 then as many of +1 (both signs flipped with `invert`), designed in initialize() from get_rate().  Its output peaks
+    positive at 1 -> 0 transitions and negative at 0 -> 1 transitions."""
+    name = "ManchesterMatchedFilterBlock"
+
+    def instantiate(self, baudrate, invert=False):
+        assert baudrate is not None, "Missing argument #1 (baudrate)"
+        self.baudrate, self.invert = baudrate, bool(invert)
+        self.taps, self.use_fft = Float32.vector(32), None          # designed in initialize()
+        self.add_type_signature([Input("in", Float32)], [Output("out", Float32)])
+
+    @staticmethod
+    def design(rate, baudrate, invert):
+        """The taps: the reference's `for i=1, symbol_period` loop runs floor(symbol_period) times."""
+        period = int(math.floor(rate / baudrate))
+        assert period >= 1, "Sample rate %g is below the baud rate %g" % (rate, baudrate)
+        sign = -1.0 if invert else 1.0
+        return np.concatenate([np.full(period, -sign), np.full(period, sign)]).astype(np.float32)
+
+    def initialize(self):
+        self.taps = Float32.vector_from_array(self.design(self.get_rate(), self.baudrate, self.invert))
+        FIRFilterBlock.initialize(self)
+
+
 class BinaryPhaseCorrectorBlock(GPUBlock):
     """binaryphasecorrector.lua:28-77: rotates a BPSK signal against the moving average of its phase, folded into
     (-pi/2, pi/2], measured every `sample_interval` samples over the last `num_samples` measurements."""
