@@ -336,12 +336,18 @@ void   lrb200_graph_destroy(lrb200_graph_t* g);
  * pending is an error (flush first), and so is a flush with no execute since the mode was set, the last flush or reset.
  * lrb200_dag_max_output is the room `y[output]` of the next execute(n) (or flush, n = 0) must have, in either mode.
  * lrb200_dag_reset waits for the slots in flight and drops them with the partial slot (the super-chunk size stays), then
- * zeroes every node's state: the DAG then computes what a fresh one does. */
+ * zeroes every node's state: the DAG then computes what a fresh one does.
+ * lrb200_dag_commit applies the DAG's rewrites (fuse != 0) to the nodes and outputs set so far: two ComplexMagnitude-behind-
+ * FIR branches (cccf, equal tap counts <= 513, D = 1) on one input meeting in a real Subtract, every port inside them read
+ * once and no DAG output, become one node `fsk_detect(M)[fused x5]`, equal to the five blocks bit for bit.  A DAG the
+ * caller does not commit is committed with fuse = 1 by its first execute, halo, seek, super-chunk size or description.
+ * Once a rewrite has renumbered the nodes, adding nodes and setting outputs are refused. */
 typedef struct lrb200_dag_s lrb200_dag_t;
 lrb200_dag_t* lrb200_dag_create(void);
 int    lrb200_dag_add_block(lrb200_dag_t* d, lrb200_block_t* q, const int* inputs, unsigned num_inputs);   /* node id or -1 */
 int    lrb200_dag_add_graph(lrb200_dag_t* d, lrb200_graph_t* g, int input);                                /* node id or -1 */
 int    lrb200_dag_set_outputs(lrb200_dag_t* d, const int* outputs, unsigned num_outputs);
+int    lrb200_dag_commit(lrb200_dag_t* d, int fuse);
 int    lrb200_dag_execute(lrb200_dag_t* d, const void* x, size_t n, void* const* y, size_t* n_out);        /* n_out[k] per output */
 int    lrb200_dag_execute_device(lrb200_dag_t* d, const void* dx, size_t n, void* const* dy, size_t* n_out); /* DEVICE in/outs, async */
 size_t lrb200_dag_max_output(const lrb200_dag_t* d, unsigned output, size_t n);

@@ -103,6 +103,7 @@ _PROTOS = {
     "lrb200_dag_add_block": (c_int, [c_void_p, c_void_p, POINTER(c_int), c_uint]),
     "lrb200_dag_add_graph": (c_int, [c_void_p, c_void_p, c_int]),
     "lrb200_dag_set_outputs": (c_int, [c_void_p, POINTER(c_int), c_uint]),
+    "lrb200_dag_commit": (c_int, [c_void_p, c_int]),
     "lrb200_dag_execute": (c_int, [c_void_p, c_void_p, c_size_t, POINTER(c_void_p), POINTER(c_size_t)]),
     "lrb200_dag_execute_device": (c_int, [c_void_p, c_void_p, c_size_t, POINTER(c_void_p), POINTER(c_size_t)]),
     "lrb200_dag_max_output": (c_size_t, [c_void_p, c_uint, c_size_t]),

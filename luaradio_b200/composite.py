@@ -928,6 +928,8 @@ class GPUDagBlock(Block):
             done.add(b)
         outs = (ctypes.c_int * len(self.ext_out))(*[ref[p] for p in self.ext_out])
         _lib.check(lib.lrb200_dag_set_outputs(d, outs, len(self.ext_out)), "dag_set_outputs")
+        if not self.fuse:                            # else the DAG commits itself, rewrites on, at its first use
+            _lib.check(lib.lrb200_dag_commit(d, 0), "dag_commit")
         if self.superchunk:
             _lib.check(lib.lrb200_dag_set_superchunk(d, self.superchunk), "dag_set_superchunk")
         self.desc = "dag{" + lib.lrb200_dag_describe(d).decode() + "}"

@@ -32,8 +32,6 @@ inline int ax_grid(long long items) {
     return (int)(blocks < 1 ? 1 : blocks);
 }
 
-enum BinOp { BIN_MUL = 0, BIN_MULCONJ = 1, BIN_ADD = 2, BIN_SUB = 3 };
-
 template <int OP>
 __device__ __forceinline__ float2 bin_c(float2 a, float2 b) {
     if constexpr (OP == BIN_MUL) return cmul(a, b);
@@ -204,40 +202,27 @@ psd1024_kernel(const void* __restrict__ xv, const float* __restrict__ window, fl
 
 }  // namespace
 
-struct BinaryBlock : Block {
-    int op;
-    bool cplx;
-    static constexpr const char* NAMES[] = {"multiply", "multiplyconjugate", "add", "subtract"};
-    BinaryBlock(int op_, bool cplx_, bool dev)
-        : Block(std::string(NAMES[op_]) + (cplx_ ? "_cc" : "_rr"), cplx_ ? 8 : 4, cplx_ ? 8 : 4, dev), op(op_), cplx(cplx_) {
-        num_inputs = 2;
-    }
-    int run(const void*, size_t, void*, size_t*, cudaStream_t) override {
-        set_error("%s needs two inputs: use lrb200_block_execute_multi", name.c_str());
-        return -1;
-    }
-    int run_multi(const void* const* dx, int nin, size_t n, void* const* dy, int nout, size_t* n_out, cudaStream_t s) override {
-        if (nin != 2 || nout != 1) { set_error("%s: expected 2 inputs and 1 output", name.c_str()); return -1; }
-        *n_out = n;
-        if (n == 0) return 0;
-        const int vec = ((reinterpret_cast<uintptr_t>(dx[0]) | reinterpret_cast<uintptr_t>(dx[1]) | reinterpret_cast<uintptr_t>(dy[0])) & 15) == 0;
-        const int grid = ax_grid((long long)n / (cplx ? 2 : 4) + 1);
+int BinaryBlock::run_multi(const void* const* dx, int nin, size_t n, void* const* dy, int nout, size_t* n_out, cudaStream_t s) {
+    if (nin != 2 || nout != 1) { set_error("%s: expected 2 inputs and 1 output", name.c_str()); return -1; }
+    *n_out = n;
+    if (n == 0) return 0;
+    const int vec = ((reinterpret_cast<uintptr_t>(dx[0]) | reinterpret_cast<uintptr_t>(dx[1]) | reinterpret_cast<uintptr_t>(dy[0])) & 15) == 0;
+    const int grid = ax_grid((long long)n / (cplx ? 2 : 4) + 1);
 #define LRB_BIN(OP)                                                                                                        \
-        if (cplx) binary_c_kernel<OP><<<grid, AX_THREADS, 0, s>>>((const float2*)dx[0], (const float2*)dx[1], (float2*)dy[0], (long long)n, vec); \
-        else binary_r_kernel<OP><<<grid, AX_THREADS, 0, s>>>((const float*)dx[0], (const float*)dx[1], (float*)dy[0], (long long)n, vec);
-        switch (op) {
-            case BIN_MUL: LRB_BIN(BIN_MUL) break;
-            case BIN_MULCONJ: LRB_BIN(BIN_MULCONJ) break;
-            case BIN_ADD: LRB_BIN(BIN_ADD) break;
-            default: LRB_BIN(BIN_SUB) break;
-        }
-#undef LRB_BIN
-        count_launch();
-        LRB_CHECK(cudaGetLastError());
-        consumed += n;
-        return 0;
+    if (cplx) binary_c_kernel<OP><<<grid, AX_THREADS, 0, s>>>((const float2*)dx[0], (const float2*)dx[1], (float2*)dy[0], (long long)n, vec); \
+    else binary_r_kernel<OP><<<grid, AX_THREADS, 0, s>>>((const float*)dx[0], (const float*)dx[1], (float*)dy[0], (long long)n, vec);
+    switch (op) {
+        case BIN_MUL: LRB_BIN(BIN_MUL) break;
+        case BIN_MULCONJ: LRB_BIN(BIN_MULCONJ) break;
+        case BIN_ADD: LRB_BIN(BIN_ADD) break;
+        default: LRB_BIN(BIN_SUB) break;
     }
-};
+#undef LRB_BIN
+    count_launch();
+    LRB_CHECK(cudaGetLastError());
+    consumed += n;
+    return 0;
+}
 
 struct DelayBlock : Block {
     long long D;

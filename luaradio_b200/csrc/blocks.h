@@ -130,6 +130,11 @@ int fir_fast_prepare(FirKind kind, const void* taps, int M, int D, bool rotate, 
 int launch_overlap_save(const FirFast& f, const void* x, const void* hist, long long n, void* y, long long first,
                         uint64_t g0, cudaStream_t s);
 int launch_delay_line(const FirFast& f, const void* x, const void* hist, long long n, void* y, cudaStream_t s);
+// the fused FSK detector (overlap-save mode IN 4): y = |x * a| - |x * b| over one complex input and one history, for two
+// complex-input single-block plans of equal length, D = 1, no translator
+int launch_fsk_detect(const FirFast& a, const FirFast& b, const void* x, const void* hist, long long n, float* y, cudaStream_t s);
+// y = |a| - |b| element-wise, as ComplexMagnitudeBlock's kernel and the real SubtractBlock's compute it
+int launch_magsub(const float2* a, const float2* b, float* y, long long n, cudaStream_t s);
 
 struct PolyTaps;  // polyphase decimator taps (tuner.cu)
 
@@ -178,6 +183,40 @@ struct FirBlock : Block {
     FirPath path(size_t n) const;     // the kernel a call of n inputs runs
     bool always_polyphase() const { return poly != nullptr && algo != LRB200_FIR_FFT; }    // path(n) for every n
     int effective_algorithm() const;  // path() of a long call as LRB200_FIR_DIRECT / FFT (lrb200_fir_get_algorithm)
+};
+
+// ComplexMagnitude behind each of two complex-tap FIRs on one input, then Subtract: y = |x * h_a| - |x * h_b| (the POCSAG
+// receiver's mark/space detector, composites/pocsagreceiver.lua:28-45), made by the device DAG's rewrite (graph.cu).  One
+// input history serves both branches.  Which kernels a call runs is decided in one place, FskDetectBlock::fused.
+struct FskDetectBlock : Block {
+    std::unique_ptr<FirBlock> fa, fb;  // the member FIRs: taps, overlap-save plans and kernel choice (their histories unused)
+    int M = 0;
+    DeviceBuffer d_hist[2];           // the last M - 1 inputs
+    int cur = 0;
+    DeviceBuffer d_branch;            // calls the fused kernel does not take: both branches' FIR outputs
+    FskDetectBlock(std::unique_ptr<FirBlock> a, std::unique_ptr<FirBlock> b, bool dev);
+    int init() override;
+    int run(const void* dx, size_t n, void* dy, size_t* n_out, cudaStream_t s) override;
+    // the cut rule's walk through the five members: Subtract (+1), ComplexMagnitude (+1), the FIR (M - 1 + 1)
+    long long memory_in() const override { return M + 1; }
+    bool fused(size_t n) const;       // a call of n inputs runs the fused kernel
+};
+
+// MultiplyBlock / MultiplyConjugateBlock / AddBlock / SubtractBlock (aux_blocks.cu)
+enum BinOp { BIN_MUL = 0, BIN_MULCONJ = 1, BIN_ADD = 2, BIN_SUB = 3 };
+struct BinaryBlock : Block {
+    int op;
+    bool cplx;
+    static constexpr const char* NAMES[] = {"multiply", "multiplyconjugate", "add", "subtract"};
+    BinaryBlock(int op_, bool cplx_, bool dev)
+        : Block(std::string(NAMES[op_]) + (cplx_ ? "_cc" : "_rr"), cplx_ ? 8 : 4, cplx_ ? 8 : 4, dev), op(op_), cplx(cplx_) {
+        num_inputs = 2;
+    }
+    int run(const void*, size_t, void*, size_t*, cudaStream_t) override {
+        set_error("%s needs two inputs: use lrb200_block_execute_multi", name.c_str());
+        return -1;
+    }
+    int run_multi(const void* const* dx, int nin, size_t n, void* const* dy, int nout, size_t* n_out, cudaStream_t s) override;
 };
 
 struct RotatorBlock : Block {

@@ -216,6 +216,60 @@ int FirBlock::run(const void* dx, size_t n, void* dy, size_t* n_out, cudaStream_
 }
 
 // ---------------------------------------------------------------------------------------------
+// Fused FSK detector: |x * h_a| - |x * h_b|
+// ---------------------------------------------------------------------------------------------
+FskDetectBlock::FskDetectBlock(std::unique_ptr<FirBlock> a, std::unique_ptr<FirBlock> b, bool dev)
+    : Block("fsk_detect(" + std::to_string(a->M) + ")", 8, 4, dev), fa(std::move(a)), fb(std::move(b)) {
+    M = fa->M;
+}
+
+int FskDetectBlock::init() { return carry(d_hist, (size_t)(M > 1 ? M - 1 : 1) * 8, cur); }
+
+// The policy: the fused kernel when both member FIRs would run the overlap-save kernel on this call, else each FIR's own
+// kernel (FirBlock::path) followed by the magnitudes and the difference, so that every call equals the unfused members'.
+bool FskDetectBlock::fused(size_t n) const {
+    return fa->path(n) == FirPath::OverlapSave && fb->path(n) == FirPath::OverlapSave;
+}
+
+int FskDetectBlock::run(const void* dx, size_t n, void* dy, size_t* n_out, cudaStream_t s) {
+    *n_out = n;
+    if (n == 0) return 0;
+    const bool one = fused(n);
+    if (!one && d_branch.capacity() < 2 * n * sizeof(float2)) {
+        LRB_CHECK(cudaStreamSynchronize(s));             // launches in flight may still read the old buffer
+        if (d_branch.reserve(2 * n * sizeof(float2)) != 0) return -1;
+    }
+    cudaStream_t side = s;
+    if (M > 1) {
+        if (n >= SIDE_STREAM_MIN) side = side_fork(s);
+        if (launch_hist_update(dx, (long long)n, d_hist[cur].get(), d_hist[cur ^ 1].get(), M - 1, 8, side) != 0) return -1;
+    }
+    const void* hist = d_hist[cur].get();
+    int rc = 0;
+    if (one) {
+        rc = launch_fsk_detect(*fa->fast, *fb->fast, dx, hist, (long long)n, (float*)dy, s);
+    } else {
+        float2* yb[2] = {d_branch.as<float2>(), d_branch.as<float2>() + n};
+        const FirBlock* f[2] = {fa.get(), fb.get()};
+        // a cccf FIR with D = 1 and M <= FFT_MAX_TAPS has no polyphase kernel and no delay line: FirBlock::run's other
+        // cases cannot occur, and are refused rather than run differently from the member
+        for (int k = 0; k < 2 && rc == 0; ++k) {
+            switch (f[k]->path(n)) {
+                case FirPath::OverlapSave: rc = launch_overlap_save(*f[k]->fast, dx, hist, (long long)n, yb[k], 0, consumed, s); break;
+                case FirPath::Direct: rc = launch_fir_generic(FIR_CCCF, dx, hist, f[k]->d_taps.get(), M, 1, 0, (long long)n, yb[k], s); break;
+                default: set_error("fsk_detect: a member FIR chose a kernel the fused node does not run"); rc = -1;
+            }
+        }
+        if (rc == 0) rc = launch_magsub(yb[0], yb[1], (float*)dy, (long long)n, s);
+    }
+    side_join(s, side);
+    if (rc != 0) return -1;
+    if (M > 1) cur ^= 1;
+    consumed += n;
+    return 0;
+}
+
+// ---------------------------------------------------------------------------------------------
 // FrequencyTranslator
 // ---------------------------------------------------------------------------------------------
 RotatorBlock::RotatorBlock(double turns_per_sample, bool dev) : Block("rotator", 8, 8, dev) {

@@ -49,6 +49,28 @@ __device__ __forceinline__ float2 cmul_conj_if(float2 a, float2 w, bool conj) {
     return ffma2(a, make_float2(w.x, w.x), t);
 }
 
+// X[k1 + 32 k2] in v[bitrev5(k2)] (lane = k1) times the tap spectrum H (1/N folded in), then the inverse transform:
+// y[n2 + 32 n1] in v[bitrev5(n1)] (lane = n2).  xch is the warp's transposition tile.
+__device__ __forceinline__ void ff_product_inverse(float2 (&v)[32], const float2* s_H, const float2* s_tw, float2* xch, int lane) {
+    // ---- multiply by the tap spectrum
+#pragma unroll
+    for (int k2 = 0; k2 < 32; ++k2) v[bitrev5(k2)] = cmul_conj_if(v[bitrev5(k2)], s_H[k2 * 32 + lane], false);
+    // ---- inverse pass 1: lane = k1, registers k2 (bit-reversed placement) -> n2 (natural)
+    fft32_br2nat<true>(v);
+    __syncwarp();                               // earlier reads of the tile are done
+#pragma unroll
+    for (int n2 = 0; n2 < 32; ++n2) {
+        float2 t = v[n2];
+        if (n2 > 0) t = cmul_conj_if(t, s_tw[n2 * 32 + lane], true);
+        xch[n2 * FF_XSTRIDE + lane] = t;
+    }
+    __syncwarp();
+#pragma unroll
+    for (int r = 0; r < 32; ++r) v[r] = xch[lane * FF_XSTRIDE + r];      // lane = n2, r = k1
+    // ---- inverse pass 2: registers k1 -> n1 (y[n2 + 32 n1] in v[bitrev5(n1)])
+    fft32_nat2br<true>(v);
+}
+
 struct FftArgs {
     const void* x;
     const void* hist;
@@ -61,6 +83,7 @@ struct FftArgs {
     long long first;          // decimation: keep outputs at input index first + j*D
     uint64_t turns_fix, g0;   // fused translator
     int M, D;
+    const float2* H2;         // IN 4: the second branch's tap spectrum
 };
 
 // a real input sample of the packed-real modes: IN 1 reads it, IN 3 takes the magnitude of a complex sample
@@ -79,6 +102,10 @@ __device__ __forceinline__ void floor_divmod(long long t, int d, long long* q, i
 // IN   0: complex in / complex out (crcf, cccf)         1: real in, two blocks packed per FFT / real out (rrrf)
 //      2: real in / complex out with complex taps (Hilbert: taps = delay + j*hilbert)
 //      3: complex in, |x| taken at the load (fused ComplexMagnitude), then as IN 1: real taps, real out
+//      4: complex in, two complex tap spectra H, H2 on one forward transform, real out |x * h| - |x * h2| (the fused
+//         FSK detector: ComplexMagnitude behind either FIR, then Subtract).  Each branch is IN 0's product and inverse
+//         transform; the spectrum X waits in a warp-private stash while the first branch runs, and the first branch's
+//         magnitudes take its place there while the second one runs.  D = 1, no translator.
 // EDGE false: interior blocks [b_lo, b_hi): all N inputs inside x, unconditional coalesced loads (one code path:
 //             guarded loads made the compiler clone the butterfly networks behind each branch);
 //      true : blocks touching the carried history (b = 0) or the end of the input (b >= b_hi), bounds-checked;
@@ -86,19 +113,25 @@ __device__ __forceinline__ void floor_divmod(long long t, int d, long long* q, i
 // ROT  (IN 0): fused FrequencyTranslator: x[i] * exp(j w (g0+i)) = P_b * (x[i] * E[i - base]); E is applied at the
 //             load, the per-block phasor P_b commutes with the (linear) filter and is applied to kept outputs only.
 // DEC  fused Downsampler: only outputs at input index first + j*D are stored, at y[j].
+// IN 4 runs one CTA per SM (its shared memory), so it asks for one: the register cap of two would make its edge kernel spill
 template <int IN, bool EDGE, bool ROT, bool DEC>
-__global__ void __launch_bounds__(FF_THREADS, 2)
+__global__ void __launch_bounds__(FF_THREADS, IN == 4 ? 1 : 2)
 fir_fft1024_kernel(const __grid_constant__ FftArgs A) {
     extern __shared__ __align__(16) float2 sm[];
     float2* s_tw = sm;                            // [k1][n2]  W1024^(k1*n2)
     float2* s_H = sm + FF_N;                      // [k2][k1]  H[k1 + 32 k2] / N
     float2* s_E = sm + 2 * FF_N;                  // [r][lane] (ROT)
+    float2* s_H2 = sm + 2 * FF_N;                 // [k2][k1]  H2[k1 + 32 k2] / N  (IN 4)
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
-    float2* xch = sm + (ROT ? 3 : 2) * FF_N + warp * FF_XCH;
+    constexpr int TABLES = (ROT || IN == 4) ? 3 : 2;
+    float2* xch = sm + TABLES * FF_N + warp * FF_XCH;
+    float2* stash = sm + TABLES * FF_N + FF_WARPS * FF_XCH + warp * FF_N;     // IN 4: [r][lane], lane-private
+    (void)stash;
     for (int i = tid; i < FF_N; i += FF_THREADS) {
         s_tw[i] = A.tw[i];
         s_H[i] = A.H[i];
         if constexpr (ROT) s_E[i] = A.E[i];
+        if constexpr (IN == 4) s_H2[i] = A.H2[i];
     }
     __syncthreads();
 
@@ -113,7 +146,7 @@ fir_fft1024_kernel(const __grid_constant__ FftArgs A) {
         const long long b = EDGE ? (wi < A.b_lo ? wi : A.b_hi + (wi - A.b_lo)) : (A.b_lo + wi);
         float2 v[32];
         // ---- load: v[r] = X[base + 32 r + lane]
-        if constexpr (IN == 0) {
+        if constexpr (IN == 0 || IN == 4) {
             const float2* x = reinterpret_cast<const float2*>(A.x);
             const float2* hist = reinterpret_cast<const float2*>(A.hist);
             const long long base = b * L - Hm1;
@@ -192,26 +225,37 @@ fir_fft1024_kernel(const __grid_constant__ FftArgs A) {
         for (int r = 0; r < 32; ++r) v[r] = xch[lane * FF_XSTRIDE + r];      // lane = k1, r = n2
         // ---- forward pass 2: registers n2 -> k2 (X[k1 + 32 k2] in v[bitrev5(k2)])
         fft32_nat2br<false>(v);
-        // ---- multiply by the tap spectrum (1/N folded in)
+        if constexpr (IN == 4) {
 #pragma unroll
-        for (int k2 = 0; k2 < 32; ++k2) v[bitrev5(k2)] = cmul_conj_if(v[bitrev5(k2)], s_H[k2 * 32 + lane], false);
-        // ---- inverse pass 1: lane = k1, registers k2 (bit-reversed placement) -> n2 (natural)
-        fft32_br2nat<true>(v);
-        __syncwarp();                               // tile reads of the forward transpose are done
-#pragma unroll
-        for (int n2 = 0; n2 < 32; ++n2) {
-            float2 t = v[n2];
-            if (n2 > 0) t = cmul_conj_if(t, s_tw[n2 * 32 + lane], true);
-            xch[n2 * FF_XSTRIDE + lane] = t;
+            for (int r = 0; r < 32; ++r) stash[r * 32 + lane] = v[r];
         }
-        __syncwarp();
-#pragma unroll
-        for (int r = 0; r < 32; ++r) v[r] = xch[lane * FF_XSTRIDE + r];      // lane = n2, r = k1
-        // ---- inverse pass 2: registers k1 -> n1 (y[n2 + 32 n1] in v[bitrev5(n1)])
-        fft32_nat2br<true>(v);
+        // ---- product with the tap spectrum and inverse transform (IN 4: the first branch's)
+        ff_product_inverse(v, s_H, s_tw, xch, lane);
 
         // ---- store the L valid outputs: block index nn = 32 n1 + lane >= M-1  ->  input-aligned index o = obase + nn
-        if constexpr (IN == 0 || IN == 2) {
+        if constexpr (IN == 4) {
+            // the first branch's magnitudes replace X in the stash as X is read back: slot r holds those of n1 = 2r, 2r + 1
+            float m[32];
+#pragma unroll
+            for (int n1 = 0; n1 < 32; ++n1) m[n1] = cmag_of(v[bitrev5(n1)]);
+#pragma unroll
+            for (int r = 0; r < 32; ++r) {
+                v[r] = stash[r * 32 + lane];
+                if (r < 16) stash[r * 32 + lane] = make_float2(m[2 * r], m[2 * r + 1]);
+            }
+            ff_product_inverse(v, s_H2, s_tw, xch, lane);
+            float* y = reinterpret_cast<float*>(A.y);
+            const long long obase = b * L - Hm1;
+#pragma unroll
+            for (int n1 = 0; n1 < 32; ++n1) {
+                const int nn = 32 * n1 + lane;
+                const long long o = obase + nn;
+                if (nn >= Hm1 && (!EDGE || o < n)) {
+                    const float2 mp = stash[(n1 / 2) * 32 + lane];
+                    __stcs(y + o, __fsub_rn((n1 & 1) ? mp.y : mp.x, cmag_of(v[bitrev5(n1)])));
+                }
+            }
+        } else if constexpr (IN == 0 || IN == 2) {
             float2* y = reinterpret_cast<float2*>(A.y);
             const long long obase = b * L - Hm1;
             if constexpr (!DEC) {
@@ -280,7 +324,9 @@ template <int IN, bool ROT, bool DEC>
 int launch_fft(const FftArgs& base_args, long long n_int, long long n_edge, cudaStream_t s) {
     static bool configured_dev[LRB_MAX_DEVICES] = {false};     // function attributes are per device
     bool& configured = configured_dev[ctx().device & (LRB_MAX_DEVICES - 1)];
-    constexpr size_t smem = (size_t)((ROT ? 3 : 2) * FF_N + FF_WARPS * FF_XCH) * sizeof(float2);
+    // IN 4 also holds a second tap spectrum and a stash per warp: 154 KiB, one CTA per SM (the others: 82 KiB, two)
+    constexpr size_t smem = IN == 4 ? (size_t)(3 * FF_N + FF_WARPS * (FF_XCH + FF_N)) * sizeof(float2)
+                                    : (size_t)((ROT ? 3 : 2) * FF_N + FF_WARPS * FF_XCH) * sizeof(float2);
     auto ki = fir_fft1024_kernel<IN, false, ROT, DEC>;
     auto ke = fir_fft1024_kernel<IN, true, ROT, DEC>;
     if (!configured) {
@@ -288,7 +334,7 @@ int launch_fft(const FftArgs& base_args, long long n_int, long long n_edge, cuda
         LRB_CHECK(cudaFuncSetAttribute(ke, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
         configured = true;
     }
-    const long long max_ctas = (long long)ctx().sm_count * 2;
+    const long long max_ctas = (long long)ctx().sm_count * (IN == 4 ? 1 : 2);
     // edge blocks on the side stream (they only overlap the interior kernel and touch disjoint outputs)
     cudaStream_t side = (n_int > 0 && n_edge > 0) ? side_fork(s) : s;
     if (n_edge > 0) {
@@ -629,21 +675,27 @@ int launch_delay_line(const FirFast& f, const void* x, const void* hist, long lo
     return 0;
 }
 
+// the interior blocks [b_lo, b_hi) of a call of n inputs, blocks of `per` outputs: b*per - (M-1) >= 0 and (b+1)*per <= n
+static void interior_blocks(long long n, int M, long long per, long long* nblocks, long long* lo, long long* hi) {
+    const long long nb = (n + per - 1) / per;
+    long long b_lo = ((long long)(M - 1) + per - 1) / per;
+    if (b_lo < 1) b_lo = 1;
+    long long b_hi = n / per;
+    if (b_hi > nb) b_hi = nb;
+    if (b_hi < b_lo) b_hi = b_lo;
+    if (b_lo > nb) { b_lo = nb; b_hi = nb; }
+    *nblocks = nb; *lo = b_lo; *hi = b_hi;
+}
+
 int launch_overlap_save(const FirFast& f, const void* x, const void* hist, long long n, void* y, long long first,
                         uint64_t g0, cudaStream_t s) {
     const int L = f.block_len();
     // blocks of L outputs; in packed-real mode one FFT covers two of them
     const long long per = (f.in_mode == 1 || f.in_mode == 3) ? 2LL * L : (long long)L;
-    const long long nblocks = (n + per - 1) / per;
-    // interior blocks [b_lo, b_hi): b*per - (M-1) >= 0  and  (b+1)*per <= n
-    long long b_lo = ((long long)(f.M - 1) + per - 1) / per;
-    if (b_lo < 1) b_lo = 1;
-    long long b_hi = n / per;
-    if (b_hi > nblocks) b_hi = nblocks;
-    if (b_hi < b_lo) b_hi = b_lo;
-    if (b_lo > nblocks) { b_lo = nblocks; b_hi = nblocks; }
+    long long nblocks, b_lo, b_hi;
+    interior_blocks(n, f.M, per, &nblocks, &b_lo, &b_hi);
     FftArgs a;
-    a.x = x; a.hist = hist; a.y = y; a.H = f.d_H.as<float2>(); a.tw = f.d_tw.as<float2>(); a.E = f.d_E.as<float2>();
+    a.x = x; a.hist = hist; a.y = y; a.H = f.d_H.as<float2>(); a.H2 = nullptr; a.tw = f.d_tw.as<float2>(); a.E = f.d_E.as<float2>();
     a.n = n; a.b_lo = b_lo; a.b_hi = b_hi; a.nwork = 0; a.first = first;
     a.turns_fix = f.rot_fix; a.g0 = g0; a.M = f.M; a.D = f.D;
     // edge work list: blocks [0, b_lo) and [b_hi, nblocks); the kernel maps e -> (e < b_lo ? e : b_hi + e - b_lo)
@@ -659,6 +711,42 @@ int launch_overlap_save(const FirFast& f, const void* x, const void* hist, long 
         default:
             return launch_fft<2, false, false>(a, n_int, n_edge, s);
     }
+}
+
+int launch_fsk_detect(const FirFast& fa, const FirFast& fb, const void* x, const void* hist, long long n, float* y,
+                      cudaStream_t s) {
+    if (fa.in_mode != 0 || fb.in_mode != 0 || fa.M != fb.M || fa.nparts != 1 || fb.nparts != 1 || fa.D != 1 || fb.D != 1 ||
+        fa.rotate || fb.rotate) {
+        set_error("fsk_detect: needs two complex-input overlap-save plans of equal length, D = 1, no translator");
+        return -1;
+    }
+    long long nblocks, b_lo, b_hi;
+    interior_blocks(n, fa.M, fa.block_len(), &nblocks, &b_lo, &b_hi);
+    FftArgs a;
+    a.x = x; a.hist = hist; a.y = y; a.H = fa.d_H.as<float2>(); a.H2 = fb.d_H.as<float2>(); a.tw = fa.d_tw.as<float2>();
+    a.E = nullptr;
+    a.n = n; a.b_lo = b_lo; a.b_hi = b_hi; a.nwork = 0; a.first = 0;
+    a.turns_fix = 0; a.g0 = 0; a.M = fa.M; a.D = 1;
+    return launch_fft<4, false, false>(a, b_hi - b_lo, b_lo + (nblocks - b_hi), s);
+}
+
+namespace {
+__global__ void __launch_bounds__(256) fsk_magsub_kernel(const float2* __restrict__ a, const float2* __restrict__ b,
+                                                         float* __restrict__ y, long long n) {
+    const long long stride = (long long)gridDim.x * blockDim.x;
+    for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += stride)
+        y[i] = __fsub_rn(cmag_of(a[i]), cmag_of(b[i]));
+}
+}  // namespace
+
+int launch_magsub(const float2* a, const float2* b, float* y, long long n, cudaStream_t s) {
+    if (n <= 0) return 0;
+    long long grid = (n + 255) / 256;
+    if (grid > (long long)ctx().sm_count * 16) grid = (long long)ctx().sm_count * 16;
+    fsk_magsub_kernel<<<(unsigned)grid, 256, 0, s>>>(a, b, y, n);
+    count_launch();
+    LRB_CHECK(cudaGetLastError());
+    return 0;
 }
 
 }  // namespace lrb

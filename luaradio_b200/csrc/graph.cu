@@ -764,6 +764,7 @@ struct PortRef {
 
 struct DagNode {
     std::unique_ptr<Block> blk;    // a block, or a committed linear Graph
+    int members = 1;               // the blocks a DAG rewrite folded into this node (the description's [fused xN])
     std::vector<PortRef> ins;
     std::vector<DeviceBuffer> out_buf;
     std::vector<size_t> out_cnt;
@@ -776,11 +777,69 @@ struct DagNode {
     long long probe = -1;          // a PLL's probe point in the first shard's run (shard_begin), or -1
 };
 
+// What a DAG rule made of the nodes around nodes[at]: one node standing for `members` blocks, fed by `in`, in the place of
+// nodes[at]; the nodes in `gone` go.  No match: node stays null.
+struct DagRewrite {
+    std::unique_ptr<Block> node;
+    PortRef in;
+    std::vector<int> gone;
+    int members = 0;
+};
+struct Dag;
+// 0 (a match or none, see out->node), or -1 with the error set
+using DagRule = int (*)(const Dag& dag, size_t at, DagRewrite* out);
+extern const DagRule DAG_RULES[1];
+
 struct Dag {
     std::vector<DagNode> nodes;
     std::vector<PortRef> outputs;  // never the DAG input
     size_t in_size = 0;
     std::string desc;
+    // commit applies the DAG rules (fuse != 0) once the nodes and outputs are known.  A DAG not committed by the caller is
+    // committed with fuse = 1 by its first run, halo, seek, super-chunk size or description.  Once a rule has rewritten
+    // nodes, node ids have changed: adding nodes or setting outputs is refused from then on.
+    bool committed = false, rewritten = false;
+    int fuse = 1;
+
+    int refuse_after_rewrite(const char* what) const {
+        if (!rewritten) return 0;
+        set_error("dag: %s after commit fused nodes (node ids have changed)", what);
+        return -1;
+    }
+    // how many node inputs and DAG outputs read port p
+    int consumers(PortRef p) const {
+        int c = 0;
+        for (const DagNode& nd : nodes)
+            for (PortRef q : nd.ins) c += (!q.is_input() && q.node == p.node && q.port == p.port);
+        for (PortRef q : outputs) c += (q.node == p.node && q.port == p.port);
+        return c;
+    }
+    int commit(int fuse_);
+    int ensure_committed() { return committed ? 0 : commit(fuse); }
+    // nodes[at] becomes rw.node, the nodes in rw.gone go, and every reference follows the renumbering
+    void apply(size_t at, DagRewrite& rw) {
+        std::vector<int> remap(nodes.size(), -1);
+        std::vector<bool> drop(nodes.size(), false);
+        for (int g : rw.gone) drop[(size_t)g] = true;
+        std::vector<DagNode> kept;
+        for (size_t j = 0; j < nodes.size(); ++j) {
+            if (drop[j]) continue;
+            remap[j] = (int)kept.size();
+            if (j != at) { kept.push_back(std::move(nodes[j])); continue; }
+            DagNode nd;
+            nd.blk = std::move(rw.node);
+            nd.members = rw.members;
+            nd.ins.assign(1, rw.in);
+            nd.out_buf.resize((size_t)nd.blk->num_outputs);
+            nd.out_cnt.assign((size_t)nd.blk->num_outputs, 0);
+            nd.out_ptr.assign((size_t)nd.blk->num_outputs, nullptr);
+            kept.push_back(std::move(nd));
+        }
+        for (DagNode& nd : kept)
+            for (PortRef& q : nd.ins) if (!q.is_input()) q.node = remap[(size_t)q.node];
+        for (PortRef& q : outputs) q.node = remap[(size_t)q.node];
+        nodes = std::move(kept);
+    }
     // host calls and super-chunk mode; the run writes each output port straight into the boundary's staging
     HostBoundary host{[this](const void* const* dx, size_t n, void* const* dy, size_t* n_out, cudaStream_t s) {
         return run_nodes(dx[0], n, dy, n_out, s);
@@ -789,6 +848,7 @@ struct Dag {
     // the boundary, sized for the current input and output ports
     HostBoundary* boundary() {
         if (nodes.empty() || outputs.empty()) { set_error("dag: no nodes / no outputs"); return nullptr; }
+        if (ensure_committed() != 0) return nullptr;
         host.in_size.assign(1, in_size);
         host.out_size.resize(outputs.size());
         for (size_t k = 0; k < outputs.size(); ++k) host.out_size[k] = out_size(k);
@@ -797,6 +857,8 @@ struct Dag {
 
     // on success the DAG owns blk; on failure the caller keeps it
     int add(Block* blk, const int* refs, unsigned nin) {
+        if (refuse_after_rewrite("add") != 0) return -1;
+        committed = false;
         DagNode nd;
         nd.blk.reset(blk);
         nd.pll = blk->as_pll();
@@ -959,6 +1021,7 @@ struct Dag {
     int plan() {
         if (sh.planned) return 0;
         if (nodes.empty() || outputs.empty()) { set_error("dag: no nodes / no outputs"); return -1; }
+        if (ensure_committed() != 0) return -1;
         sh.plls.clear();
         std::vector<Rate> rate(nodes.size());                  // total rate at each node's output
         for (size_t i = 0; i < nodes.size(); ++i) {
@@ -1005,6 +1068,7 @@ struct Dag {
     }
 
     int seek(uint64_t g) {
+        if (ensure_committed() != 0) return -1;
         const std::vector<uint64_t> idx = in_index(g);
         for (size_t i = 0; i < nodes.size(); ++i)
             if (nodes[i].blk->seek(idx[i]) != 0) return -1;
@@ -1158,6 +1222,92 @@ struct Dag {
         return rerun ? 1 : 0;
     }
 };
+
+// ---- device DAG rewrites: one rule function per rewrite, tried at every node when the DAG is committed ------------------
+
+// The FIR -> ComplexMagnitude branch whose magnitude is port p: a committed graph node `fir | cmag`, or a FIR node read only
+// by a magnitude node.  The FIR is cccf, D = 1, no fused translator, M <= FFT_MAX_TAPS; no port inside the branch has
+// another reader or is a DAG output.
+struct FskBranch {
+    FirBlock* fir = nullptr;
+    PortRef in;                      // what the FIR reads
+    std::vector<int> nodes;
+};
+static bool fsk_branch(const Dag& d, PortRef p, FskBranch* b) {
+    if (p.is_input() || d.consumers(p) != 1) return false;
+    const DagNode& m = d.nodes[(size_t)p.node];
+    C2fBlock* mag = nullptr;
+    if (Graph* g = dynamic_cast<Graph*>(m.blk.get())) {
+        if (g->stages.size() != 2) return false;
+        b->fir = dynamic_cast<FirBlock*>(g->stages[0]);
+        mag = dynamic_cast<C2fBlock*>(g->stages[1]);
+        b->in = m.ins[0];
+        b->nodes = {p.node};
+    } else if ((mag = dynamic_cast<C2fBlock*>(m.blk.get())) != nullptr) {
+        const PortRef q = m.ins[0];
+        if (q.is_input() || d.consumers(q) != 1) return false;
+        b->fir = dynamic_cast<FirBlock*>(d.nodes[(size_t)q.node].blk.get());
+        b->in = d.nodes[(size_t)q.node].ins[0];
+        b->nodes = {q.node, p.node};
+    }
+    const FirBlock* f = b->fir;
+    return mag && mag->op == 0 && f && f->kind == FIR_CCCF && f->D == 1 && !f->rotate && f->M <= FFT_MAX_TAPS && f->fast;
+}
+
+// ComplexBandpass(h_a) -> ComplexMagnitude and ComplexBandpass(h_b) -> ComplexMagnitude on one input, into Subtract's in1
+// and in2  =>  FskDetectBlock, |x * h_a| - |x * h_b| in one kernel (the POCSAG receiver's mark/space detector,
+// composites/pocsagreceiver.lua:28-45): the input is read once, and neither the two complex FIR outputs nor the two
+// magnitudes go through HBM.  Any two tap sets of equal length; the FIRs' algorithm settings carry over.
+static int fuse_fsk_detector(const Dag& d, size_t at, DagRewrite* out) {
+    const DagNode& sub = d.nodes[at];
+    const BinaryBlock* bin = dynamic_cast<const BinaryBlock*>(sub.blk.get());
+    if (!bin || bin->op != BIN_SUB || bin->cplx) return 0;
+    FskBranch br[2];
+    if (!fsk_branch(d, sub.ins[0], &br[0]) || !fsk_branch(d, sub.ins[1], &br[1])) return 0;
+    if (br[0].fir == br[1].fir || br[0].fir->M != br[1].fir->M) return 0;
+    if (br[0].in.node != br[1].in.node || br[0].in.port != br[1].in.port) return 0;
+    std::unique_ptr<FirBlock> member[2];
+    for (int k = 0; k < 2; ++k) {
+        const FirBlock& f = *br[k].fir;
+        member[k] = make_block<FirBlock>(FIR_CCCF, f.h_taps.data(), (unsigned)f.M, 1u, true);
+        if (!member[k] || member[k]->set_algorithm(f.algo) != 0) return -1;
+    }
+    out->node = make_block<FskDetectBlock>(std::move(member[0]), std::move(member[1]), true);
+    if (!out->node) return -1;
+    out->in = br[0].in;
+    out->gone = br[0].nodes;
+    out->gone.insert(out->gone.end(), br[1].nodes.begin(), br[1].nodes.end());
+    out->members = 5;
+    return 0;
+}
+
+const DagRule DAG_RULES[1] = {fuse_fsk_detector};
+
+int Dag::commit(int fuse_) {
+    if (rewritten && !fuse_) { set_error("dag: commit(0) after commit fused nodes"); return -1; }
+    fuse = fuse_;
+    if (fuse && !outputs.empty()) {
+        for (size_t i = 0; i < nodes.size(); ++i)
+            for (DagRule rule : DAG_RULES) {
+                DagRewrite rw;
+                if (rule(*this, i, &rw) != 0) return -1;
+                if (!rw.node) continue;
+                apply(i, rw);
+                rewritten = true;
+                sh.planned = false;
+                i = (size_t)-1;              // from the start: the renumbered nodes may match again
+                break;
+            }
+    }
+    desc.clear();
+    for (const DagNode& nd : nodes) {
+        if (!desc.empty()) desc += " ; ";
+        desc += nd.blk->name;
+        if (nd.members > 1) desc += "[fused x" + std::to_string(nd.members) + "]";
+    }
+    committed = true;
+    return 0;
+}
 
 }  // namespace lrb
 
@@ -1338,12 +1488,20 @@ int lrb200_dag_add_graph(lrb200_dag_t* d, lrb200_graph_t* g, int input) {
 int lrb200_dag_set_outputs(lrb200_dag_t* d, const int* outputs, unsigned num_outputs) {
     if (!d || !outputs || !num_outputs) { set_error("dag_set_outputs: null argument"); return -1; }
     if (d->d.host.samples) { set_error("dag_set_outputs: the super-chunk slots are sized for the outputs; set them first"); return -1; }
+    if (d->d.refuse_after_rewrite("set_outputs") != 0) return -1;
     std::vector<PortRef> refs(num_outputs);
     for (unsigned k = 0; k < num_outputs; ++k)
         if (d->d.decode(outputs[k], &refs[k]) != 0) { set_error("dag_set_outputs: bad reference %d", outputs[k]); return -1; }
     d->d.outputs = std::move(refs);
     d->d.sh.planned = false;
+    d->d.committed = false;
     return 0;
+}
+
+int lrb200_dag_commit(lrb200_dag_t* d, int fuse) {
+    if (!d) { set_error("null dag"); return -1; }
+    if (d->d.nodes.empty() || d->d.outputs.empty()) { set_error("dag: no nodes / no outputs"); return -1; }
+    return d->d.commit(fuse);
 }
 
 int lrb200_dag_execute(lrb200_dag_t* d, const void* x, size_t n, void* const* y, size_t* n_out) {
@@ -1354,7 +1512,7 @@ int lrb200_dag_execute(lrb200_dag_t* d, const void* x, size_t n, void* const* y,
 
 int lrb200_dag_execute_device(lrb200_dag_t* d, const void* dx, size_t n, void* const* dy, size_t* n_out) {
     if (!d || !dy || !n_out || (n && !dx)) { set_error("dag_execute_device: null argument"); return -1; }
-    if (d->d.host.refuse_direct("dag", "execute_device") != 0) return -1;
+    if (d->d.host.refuse_direct("dag", "execute_device") != 0 || d->d.ensure_committed() != 0) return -1;
     return d->d.run_nodes(dx, n, dy, n_out, ctx().stream);
 }
 
@@ -1415,7 +1573,12 @@ int lrb200_dag_shard_end(lrb200_dag_t* d, const void* left_records, unsigned num
     return d->d.shard_end((const PllShardRecord*)left_records, num_left, dy, n_out, record_out, record_bytes);
 }
 
-const char* lrb200_dag_describe(const lrb200_dag_t* d) { return d ? d->d.desc.c_str() : ""; }
+const char* lrb200_dag_describe(const lrb200_dag_t* d) {
+    if (!d) return "";
+    Dag& dag = const_cast<lrb200_dag_t*>(d)->d;          // describing commits, as lrb200_graph_describe does
+    if (!dag.nodes.empty() && !dag.outputs.empty() && dag.ensure_committed() != 0) return "";
+    return dag.desc.c_str();
+}
 
 void lrb200_dag_destroy(lrb200_dag_t* d) { delete d; }
 
